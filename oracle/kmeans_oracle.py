@@ -40,18 +40,53 @@ def max_sim(data, cent, distance="euclidean", chunk=4096):
 
 
 def compute_centroids(data, labels, k):
-    """data [l, d, n], labels [l, n] -> centroids [l, d, k] (member mean in float64, empty cluster -> 0)."""
+    """data [l, d, n], labels [l, n] -> centroids [l, d, k] (member mean in float64, empty cluster -> 0).
+    Labels outside [0, k) belong to no cluster (compute_centroids.cu:61-64 skips them)."""
     data = np.asarray(data, np.float32)
+    labels = np.asarray(labels, np.int64)
     l, d, n = data.shape
     out = np.zeros((l, d, k), np.float64)
     for li in range(l):
-        cnt = np.bincount(labels[li], minlength=k).astype(np.float64)
+        ok = (labels[li] >= 0) & (labels[li] < k)
+        lab = labels[li][ok]
+        cnt = np.bincount(lab, minlength=k).astype(np.float64)
         for e in range(d):
-            out[li, e] = np.bincount(labels[li], weights=data[li, e].astype(np.float64), minlength=k)
+            out[li, e] = np.bincount(lab, weights=data[li, e][ok].astype(np.float64), minlength=k)
         nz = cnt > 0
         out[li][:, nz] /= cnt[nz]
         out[li][:, ~nz] = 0
     return out.astype(np.float32)
+
+
+def compute_centroids_seq(data, labels, k):
+    """data [l, d, n], labels [l, n] -> centroids [l, d, k] in the arithmetic the GPU update promises: each member sum
+    is taken in fp32, starting from 0 and adding one member at a time in point order; the mean is fp32(sum) /
+    fp32(count), rounded once; an empty cluster is 0; labels outside [0, k) are ignored.  That is a fixed function of
+    the inputs, so the GPU kernels must match it bit for bit.
+
+    Vectorised over clusters: step r adds, for every cluster at once, its member of rank r (its r-th point in point
+    order), so the loop runs max(count) times, not n times."""
+    data = np.asarray(data, np.float32)
+    labels = np.asarray(labels, np.int64)
+    l, d, n = data.shape
+    out = np.zeros((l, d, k), np.float32)
+    for li in range(l):
+        pts = np.nonzero((labels[li] >= 0) & (labels[li] < k))[0]
+        if len(pts) == 0:
+            continue
+        lab = labels[li][pts]
+        pts = pts[np.argsort(lab, kind="stable")]               # grouped by cluster, point order kept inside each
+        cnt = np.bincount(lab, minlength=k)
+        start = np.concatenate(([0], np.cumsum(cnt)[:-1]))      # first sorted position of each cluster
+        by_cnt = np.argsort(-cnt, kind="stable")                # clusters with a member of rank r: a prefix of by_cnt
+        cnt_desc = cnt[by_cnt]
+        sums = np.zeros((d, k), np.float32)
+        for r in range(int(cnt_desc[0])):
+            cl = by_cnt[:np.searchsorted(-cnt_desc, -r, side="left")]   # clusters with count > r
+            sums[:, cl] += data[li][:, pts[start[cl] + r]]      # fp32 + fp32, rounded once
+        nz = cnt > 0
+        out[li][:, nz] = sums[:, nz] / cnt[nz].astype(np.float32)
+    return out
 
 
 def pq_decode(codebook, code):

@@ -41,9 +41,12 @@ if "c5" in which or "centroids" in which:
             out[name] = {"ms": ms, "algorithmic_GB": byts / 1e9, "GBps": byts / ms / 1e6, "frac_of_hbm_peak": byts / ms / 1e6 / peak,
                          "tflops_gemm_form": 2.0 * l * n * d * k / ms / 1e9, "kernel": kern}
             print(out[name], flush=True)
-        lt = T.fn.max_sim(data[:2], cent[:2], exact=False)[1]
-        le = T.fn.max_sim(data[:2], cent[:2], exact=True)[1]
+        st, lt = T.fn.max_sim(data[:2], cent[:2], exact=False)          # exact fp32 similarity of the chosen centroid
+        se, le = T.fn.max_sim(data[:2], cent[:2], exact=True)
         out["c5_label_agreement_tc_vs_exact"] = float((lt == le).float().mean())
+        diff = lt != le                                                  # where labels differ: how much worse the choice is
+        out["c5_max_rel_sim_gap_where_labels_differ"] = float(((se - st) / se.abs())[diff].max()) if diff.any() else 0.0
+        print({k: out[k] for k in ("c5_label_agreement_tc_vs_exact", "c5_max_rel_sim_gap_where_labels_differ")}, flush=True)
     if "centroids" in which:
         lab = T.fn.max_sim(data, cent)[1]
         ms = timeit(lambda: T.fn.compute_centroids(data, lab, k), reps=3, warm=1)

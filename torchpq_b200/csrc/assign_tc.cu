@@ -93,6 +93,29 @@ __device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], const uint32
       : "memory");
 }
 
+// Arg-max key of (score, column j < 256): the score with its 8 low mantissa bits replaced by an index field (a
+// perturbation below 2^-15 relative, far below the TF32 rounding of the score itself), so one fmaxf per column replaces
+// compare + two selects and the larger key always has the larger truncated score.  Among equal truncated scores the
+// LOWEST column has the largest key, for either sign: a positive float grows with its low bits, so the field is
+// 255 - j; a negative one shrinks, so the field is (255 - j) ^ 255 = j.  (The 8 masked bits still separate every two
+// scores that differ by 2^-3 or more while |score| < 2^13.)
+// Two instructions: PRMT = bytes 3..1 of the score and, as byte 0, its sign bit replicated (0x00 or 0xFF); LOP3 = XOR
+// with rcol = 255 ^ j (= 255 - j), which the caller splits into a per-thread register and an immediate.
+// A score of -0 would lose to +0 here, but the accumulator never holds -0: its last MMA adds the bias K-block, six of
+// whose products are 0 * 0 = +0, and the tensor core returns +0 for an exact-zero sum even when every other product
+// is -0 (test_max_sim_tensor_core_signed_zero_ties pins that on the GPU), so ties at zero are ties of +0.  (Turning -0
+// into +0 here, score + 0, costs one FADD per column, about 10 % of the kernel at C5.)
+__device__ __forceinline__ float argmax_key(float score, uint32_t rcol /* 255 ^ j */) {
+  uint32_t u;
+  asm("prmt.b32 %0, %1, 0, 0x321B;" : "=r"(u) : "r"(__float_as_uint(score)));
+  return __uint_as_float(u ^ rcol);
+}
+// the column j of an arg-max key: undoes the sign-dependent index field
+__device__ __forceinline__ int argmax_key_column(float key) {
+  const uint32_t u = __float_as_uint(key);
+  return 255 - (int)((u ^ (uint32_t)((int32_t)u >> 31)) & 0xFFu);
+}
+
 struct TcParams {
   int l, d, n, k;
   int nch;                       // 64-centroid chunks: N of the problem = 64 * nch >= k
@@ -210,15 +233,13 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, TcParams P) {
       }
       const float one = tq < 2 ? 1.f : 0.f;                               // A columns 0, 1 of the bias K-block = 1
       const uint32_t ones[4] = {__float_as_uint(one), __float_as_uint(one), 0u, 0u};
-      // Packed arg-max: the column index inside its 64-column chunk rides in the 8 low mantissa bits of the score (a
-      // perturbation of 2^-15 relative, far below the TF32 rounding of the score itself), so one LOP + one FMNMX per
-      // column replace compare + two selects; 63 - j: among equal truncated positive scores the lowest column wins.
-      // Chunks are then taken in column order and a later chunk wins only when its packed key is strictly larger.
+      // Packed arg-max (argmax_key): the column index rides in the 8 low mantissa bits of the score, so a running fmaxf
+      // over the packed keys of all columns and chunks is the arg-max with lowest-index ties.
       // Accumulator layout: acc[h][4i + {0,1}] = row r0, columns 64 ch + 8 i + 2 tq + {0,1}; acc[h][4i + {2,3}] = row
       // r1, same columns.  Two 64-column chunks per pass keep the accumulators at 64 registers.
-      float b0 = -3.0e38f, b1 = -3.0e38f;                                 // not -inf: index bits OR-ed into -inf make a NaN
-      int bi0 = 0, bi1 = 0;
-      const uint32_t base = 63u - 2u * (uint32_t)tq;
+      float b0 = -3.0e38f, b1 = -3.0e38f;                                 // below every key (a padded column's is ~-1e30)
+      // 255 ^ column: columns 64 ch + 8 i + 2 tq + {0,1} have disjoint bit fields, so 255 ^ j = base ^ (64 ch + 8 i + b)
+      const uint32_t base = 255u ^ (2u * (uint32_t)tq);
       #pragma unroll
       for (int c0 = 0; c0 < NCH; c0 += 2) {
         const int nh = NCH - c0 < 2 ? 1 : 2;                              // compile-time after unrolling
@@ -243,27 +264,22 @@ assign_tc_kernel(const __grid_constant__ CUtensorMap map_x, TcParams P) {
           float cb0 = -3.0e38f, cb1 = -3.0e38f;
           #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            const uint32_t i0 = base - (uint32_t)(8 * i), i1 = i0 - 1u;
-            cb0 = fmaxf(cb0, fmaxf(__uint_as_float((__float_as_uint(acc[h][4 * i + 0]) & 0xFFFFFF00u) | i0),
-                                   __uint_as_float((__float_as_uint(acc[h][4 * i + 1]) & 0xFFFFFF00u) | i1)));
-            cb1 = fmaxf(cb1, fmaxf(__uint_as_float((__float_as_uint(acc[h][4 * i + 2]) & 0xFFFFFF00u) | i0),
-                                   __uint_as_float((__float_as_uint(acc[h][4 * i + 3]) & 0xFFFFFF00u) | i1)));
+            const uint32_t i0 = base ^ (uint32_t)(64 * (c0 + h) + 8 * i), i1 = i0 ^ 1u;
+            cb0 = fmaxf(cb0, fmaxf(argmax_key(acc[h][4 * i + 0], i0), argmax_key(acc[h][4 * i + 1], i1)));
+            cb1 = fmaxf(cb1, fmaxf(argmax_key(acc[h][4 * i + 2], i0), argmax_key(acc[h][4 * i + 3], i1)));
           }
-          #pragma unroll
-          for (int o = 1; o <= 2; o <<= 1) {                              // the 4 threads of a quad share rows r0, r1
-            cb0 = fmaxf(cb0, __shfl_xor_sync(0xffffffffu, cb0, o));
-            cb1 = fmaxf(cb1, __shfl_xor_sync(0xffffffffu, cb1, o));
-          }
-          const int cbase = 64 * (c0 + h) + 63;
-          if (cb0 > b0) { b0 = cb0; bi0 = cbase - (int)(__float_as_uint(cb0) & 0xFFu); }
-          if (cb1 > b1) { b1 = cb1; bi1 = cbase - (int)(__float_as_uint(cb1) & 0xFFu); }
+          b0 = fmaxf(b0, cb0);
+          b1 = fmaxf(b1, cb1);
         }
       }
       #pragma unroll
-      for (int o = 1; o <= 2; o <<= 1) {
+      for (int o = 1; o <= 2; o <<= 1) {                                  // the 4 threads of a quad share rows r0, r1
+        b0 = fmaxf(b0, __shfl_xor_sync(0xffffffffu, b0, o));
+        b1 = fmaxf(b1, __shfl_xor_sync(0xffffffffu, b1, o));
         x2a += __shfl_xor_sync(0xffffffffu, x2a, o);
         x2b += __shfl_xor_sync(0xffffffffu, x2b, o);
       }
+      const int bi0 = argmax_key_column(b0), bi1 = argmax_key_column(b1);
       // finisher: threads tq = 0, 2 take row r0, tq = 1, 3 row r1 (all compute: no divergent path before the next
       // tile's wgmma), tq = 0, 1 store
       {

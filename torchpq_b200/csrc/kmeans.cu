@@ -386,7 +386,8 @@ extern "C" size_t tpq_compute_centroids_workspace_bytes(int l, int k) { (void)l;
 
 extern "C" int tpq_compute_centroids(const float* data, const int64_t* labels, int l, int d, int64_t n, int k,
                                      float* centroids, void* ws, size_t ws_bytes, void* stream) {
-  TPQ_REQUIRE(data && labels && centroids, "tpq_compute_centroids: null pointer");
+  // (an empty tensor may have no storage: with n = 0 only the centroids are touched)
+  TPQ_REQUIRE(centroids && (n == 0 || (data && labels)), "tpq_compute_centroids: null pointer");
   TPQ_REQUIRE(l > 0 && d > 0 && n >= 0 && k > 0 && n <= 0x7fffffffll && l <= 65535, "tpq_compute_centroids: bad sizes");
   (void)ws; (void)ws_bytes;
   cudaStream_t st = (cudaStream_t)stream;
