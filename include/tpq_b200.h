@@ -29,7 +29,9 @@ typedef enum {
   TPQ_ERR_CUDA = -4          /* a CUDA runtime call failed (message carries cudaGetErrorString) */
 } tpq_status;
 
-enum { TPQ_METRIC_EUCLIDEAN = 0, TPQ_METRIC_COSINE = 1 };
+/* MANHATTAN exists for k-means assignment only (tpq_max_sim, tpq_kmeans_assign, exact kernel); every LUT, relayout and
+ * search entry point rejects it: the index is defined for euclidean and cosine. */
+enum { TPQ_METRIC_EUCLIDEAN = 0, TPQ_METRIC_COSINE = 1, TPQ_METRIC_MANHATTAN = 2 };
 
 /* Index state read by search.  Field-for-field the buffers of the reference's
  * CellContainer / BaseContainer / codecs (container/CellContainer.py:46-81,
@@ -148,7 +150,8 @@ int tpq_ivfpq_search_cells(const tpq_index* index, const float* x_dn, const int6
  * tpq_max_sim: MultiKMeans assignment, MaxSimCuda(dim=2, mode "tn") (kernels/MaxSimCuda.py:184-238,
  *   kernels/cuda/max_sim.cu:182-309; caller clustering/MultiKMeans.py:314-333):
  *   data [l, d, n], centroids [l, d, k] -> maxsims [l, n] f32, labels [l, n] i64.
- *   metric EUCLIDEAN: sum_e -(x-c)^2 (direct form, max_sim.cu:78-98); COSINE: sum_e x*c ("inner").
+ *   metric EUCLIDEAN: sum_e -(x-c)^2 (direct form, max_sim.cu:78-98); COSINE: sum_e x*c ("inner");
+ *   MANHATTAN: sum_e -|x-c| (max_sim.cu:100-120, exact kernel only).
  *   Ties: lowest centroid index (the reference's cross-tile label write is racy, max_sim.cu:173-178).
  * tpq_compute_centroids: ComputeCentroidsCuda (kernels/ComputeCentroidsCuda.py:43-81, kernels/cuda/compute_centroids.cu:9-86):
  *   data [l, d, n], labels [l, n] i64 -> centroids [l, d, k] = member mean, 0 for an empty cluster; every member sum is
@@ -161,6 +164,25 @@ int tpq_ivfpq_search_cells(const tpq_index* index, const float* x_dn, const int6
  * in fp32 for the chosen centroid; exact == 0 -> 2*score - |x|^2 from the TF32 score (~1e-3 relative). */
 int tpq_max_sim(const float* data, const float* centroids, int l, int d, int64_t n, int k, int metric,
                 int exact, float* maxsims, int64_t* labels, void* stream);
+/* tpq_kmeans_assign: the assignment step of KMeans / MultiKMeans (clustering/KMeans.py, MultiKMeans.py) for every k and
+ *   d: data [l, d, n], centroids [l, d, k] -> maxsims [l, n] f32, labels [l, n] i64, metric as tpq_max_sim (MANHATTAN
+ *   included).  Dispatch, first match:
+ *     - euclidean, d % 8 == 0, d <= 64, 8 <= k <= 256, k % 4 == 0, n % 4 == 0, n >= 128, 16-byte-aligned data and
+ *       centroids: the TF32 wgmma kernel of tpq_max_sim (all centroids resident in shared memory);
+ *     - euclidean or cosine, d % 8 == 0, 8 <= d <= 256, 8 <= k <= 2^20, n % 4 == 0, 16-byte-aligned data and
+ *       centroids: the TF32 wgmma kernel that streams the centroids (needs the workspace);
+ *     - otherwise (manhattan included) the exact fp32 kernel of tpq_max_sim(exact == 1), bit for bit.
+ *   On the TF32 kernels labels may differ from the exact ones only between centroids closer than TF32 rounding; ties of
+ *   the TF32 score go to the lowest index.  Cosine scores are inner products: normalise data and centroids first.
+ *   maxsims: exact_values != 0 -> recomputed exactly in fp32 for the chosen centroid, in the exact kernel's order
+ *   (bit-identical to it wherever the labels agree; like tpq_max_sim's exact == 2); exact_values == 0 -> derived from
+ *   the TF32 score, 2*score - |x|^2 (euclidean) or score (cosine), ~1e-3 relative (like exact == 0).  The exact kernel
+ *   always writes exact values.
+ *   ws: at least tpq_kmeans_assign_workspace_bytes(l, d, k) bytes, 16-byte aligned (0 bytes, ws may be NULL, when
+ *   d or k is outside the streaming kernel's range); TPQ_ERR_WORKSPACE when the streaming kernel needs more. */
+size_t tpq_kmeans_assign_workspace_bytes(int l, int d, int k);
+int tpq_kmeans_assign(const float* data, const float* centroids, int l, int d, int64_t n, int k, int metric,
+                      int exact_values, float* maxsims, int64_t* labels, void* ws, size_t ws_bytes, void* stream);
 size_t tpq_compute_centroids_workspace_bytes(int l, int k);
 int tpq_compute_centroids(const float* data, const int64_t* labels, int l, int d, int64_t n, int k,
                           float* centroids, void* ws, size_t ws_bytes, void* stream);

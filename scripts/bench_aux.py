@@ -1,5 +1,6 @@
 """Secondary measurements on one H100 (results -> aux_bench.json, see the end of the file):
-C5 MultiKMeans assignment (GB/s vs HBM roofline), compute_centroids, pq_decode, and search QPS on C2 / C4.
+C5 MultiKMeans assignment (GB/s vs HBM roofline), compute_centroids, pq_decode, search QPS on C2 / C4, and (`kmeans`)
+the KMeans assignment for large k and d (TFLOP/s vs the TF32 data-sheet rate), its centroid update and a full fit.
 CUDA events, 3 warm-ups, inputs larger than L2 where the workload allows."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -25,7 +26,55 @@ def timeit(fn, reps=5, warm=3):
     return e0.elapsed_time(e1) / reps
 
 
+def card():
+    """GPU name and enforced power limit, recorded beside the numbers they qualify."""
+    import subprocess
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+        return {"gpu_name": q[0], "power_limit_w": float(q[1])}
+    except Exception as e:                                             # the numbers stay, marked as unqualified
+        return {"gpu_name": torch.cuda.get_device_name(0), "power_limit_w": None, "note": repr(e)}
+
+
 which = sys.argv[1:] or ["c5", "centroids", "decode", "c2", "c4"]
+if "kmeans" in which:
+    # KMeans at the C3 coarse-quantizer shape and the reference benchmark's largest shape (benchmark/turing/kmeans):
+    # assignment on the streaming TF32 wgmma kernel vs the exact fp32 kernel, the centroid update, and a full fit by
+    # the reference benchmark's protocol (15 iterations, tol = 0, random init).
+    TF32_PEAK = 495.0                                                  # H100 SXM dense TF32 data-sheet TFLOP/s
+    res = {"card": card()}
+    for l, d, n, k in ((1, 128, 1 << 20, 4096), (1, 256, 1 << 20, 16384)):
+        torch.manual_seed(0)
+        data = torch.randn(l, d, n, device=dev)
+        cent = data[:, :, :k].contiguous()
+        flop = 2.0 * l * n * d * k
+        r = {"shape_l_d_n_k": [l, d, n, k], "gemm_form_tflop": flop / 1e12}
+        for name, f in (("tf32_wide", lambda: T.fn.kmeans_assign(data, cent, exact_values=False)),
+                        ("tf32_wide_exact_values", lambda: T.fn.kmeans_assign(data, cent, exact_values=True)),
+                        ("exact_fp32", lambda: T.fn.max_sim(data, cent, exact=True))):
+            ms = timeit(f, reps=3, warm=1)
+            r[name] = {"ms": ms, "tflops_gemm_form": flop / ms / 1e9, "frac_of_tf32_peak": flop / ms / 1e9 / TF32_PEAK}
+        se, le = T.fn.max_sim(data, cent, exact=True)
+        st, lt = T.fn.kmeans_assign(data, cent, exact_values=True)
+        diff = lt != le
+        r["label_agreement_vs_exact"] = float((~diff).float().mean())
+        r["max_rel_sim_gap_where_labels_differ"] = float(((se - st) / se.abs())[diff].max()) if diff.any() else 0.0
+        r["maxsims_bit_identical_where_labels_agree"] = bool(torch.equal(st[~diff], se[~diff]))
+        ms = timeit(lambda: T.fn.compute_centroids(data, le, k), reps=3, warm=1)
+        r["compute_centroids_ms"] = ms
+        x = data[0]
+        km = T.KMeans(k, max_iter=15, tol=0.0, init_mode="random")
+        km.fit(x)                                                      # warm-up
+        torch.cuda.synchronize(); t0 = time.perf_counter()
+        km.fit(x)
+        torch.cuda.synchronize()
+        r["kmeans_fit_15_iter_s"] = time.perf_counter() - t0
+        r["kmeans_fit_iterations"] = km.n_iter_
+        out[f"kmeans_d{d}_k{k}"] = r
+        print(r, flush=True)
+        del data, cent, se, le, st, lt, x
+    out["kmeans_card"] = res["card"]
 if "c5" in which or "centroids" in which:
     l, d, n, k = 64, 64, 1_000_000, 256
     data = torch.randn(l, d, n, device=dev)

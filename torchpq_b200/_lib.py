@@ -20,7 +20,7 @@ TPQ_ERR_UNSUPPORTED = -2
 TPQ_ERR_WORKSPACE = -3
 TPQ_ERR_CUDA = -4
 
-METRIC = {"euclidean": 0, "cosine": 1}
+METRIC = {"euclidean": 0, "cosine": 1, "manhattan": 2}   # manhattan: k-means assignment only
 
 
 class TpqIndex(C.Structure):
@@ -62,6 +62,8 @@ SIGNATURES = {
     "tpq_part2_scan_bytes": (_SZ, [_I, _I]),
     "tpq_relayout_part2": (_I, [_P, _P, _I, _I, _I, _P, _P]),
     "tpq_max_sim": (_I, [_P, _P, _I, _I, _I64, _I, _I, _I, _P, _P, _P]),
+    "tpq_kmeans_assign_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "tpq_kmeans_assign": (_I, [_P, _P, _I, _I, _I64, _I, _I, _I, _P, _P, _P, _SZ, _P]),
     "tpq_compute_centroids_workspace_bytes": (_SZ, [_I, _I]),
     "tpq_compute_centroids": (_I, [_P, _P, _I, _I, _I64, _I, _P, _P, _SZ, _P]),
     "tpq_pq_decode": (_I, [_P, _P, _I, _I, _I64, _P, _P]),

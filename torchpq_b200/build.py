@@ -43,7 +43,8 @@ def _init_centroids(data: torch.Tensor, k: int, seed: int) -> torch.Tensor:
 
 
 def fit(data: torch.Tensor, k: int, max_iter: int, tol: float = 1e-4, n_redo: int = 1, seed: int = 0,
-        centroids: torch.Tensor | None = None, distance: str = "euclidean", exact: bool = False):
+        centroids: torch.Tensor | None = None, distance: str = "euclidean", exact: bool = False,
+        kmeans_assign: bool = False, init=None):
     """MultiKMeans.fit (clustering/MultiKMeans.py:415-453; KMeans.fit, KMeans.py:399-438, is the l = 1 case):
     l independent k-means over data [l, d, n].  Per redo: Lloyd iterations until `error = sum((new - old)^2) <= tol`
     (calculate_error, :143-149 -- a SUM of squares over all l*d*k entries, not a mean shift) or max_iter; the redo
@@ -51,17 +52,28 @@ def fit(data: torch.Tensor, k: int, max_iter: int, tol: float = 1e-4, n_redo: in
     As in the reference the returned labels are those of the last assignment, i.e. relative to the centroids BEFORE
     the final update.  exact=True: the reference's fp32 assignment arithmetic bit for bit (max_sim.cu:78-98);
     exact=False: TF32 tensor-core assignment where the shape allows (labels can differ between near-equidistant
-    centroids only)."""
+    centroids only).
+    kmeans_assign=True (the Lloyd iterations of clustering.KMeans / MultiKMeans): the assignment is
+    fn.kmeans_assign, i.e. TF32 tensor cores for every shape one of its kernels takes, cosine included, and distance
+    may also be "manhattan" (exact kernel); `exact` is then ignored.  init(data, k, seed) -> centroids replaces the
+    random initialisation (kmeans++)."""
     from . import fn
     assert data.dim() == 3 and data.is_contiguous(), "use .contiguous()"                  # MultiKMeans.py:421
-    assert distance in ("euclidean", "cosine")
+    assert distance in (("euclidean", "cosine", "manhattan") if kmeans_assign else ("euclidean", "cosine"))
+    init = init or _init_centroids
     best = None
     best_inertia = 1e32
     for redo in range(n_redo):
-        cent = centroids if (centroids is not None and redo == 0) else _init_centroids(data, k, seed + redo)
+        cent = centroids if (centroids is not None and redo == 0) else init(data, k, seed + redo)
         n_iter = 0
         for _ in range(max_iter):
-            if distance == "cosine":                                    # get_labels, MultiKMeans.py:314-333
+            if kmeans_assign:
+                x, c = data, cent.contiguous()
+                if distance == "cosine":                                # normalised out of place (the caller's tensors stay)
+                    x = data / (data.norm(dim=-2, keepdim=True) + 1e-8)
+                    c = cent / (cent.norm(dim=-2, keepdim=True) + 1e-8)
+                maxsims, labels = fn.kmeans_assign(x, c.contiguous(), distance, exact_values=n_redo > 1)
+            elif distance == "cosine":                                  # get_labels, MultiKMeans.py:314-333
                 dn = data / (data.norm(dim=-2, keepdim=True) + 1e-8)
                 cn = cent / (cent.norm(dim=-2, keepdim=True) + 1e-8)
                 maxsims, labels = fn.max_sim(dn.contiguous(), cn.contiguous(), "cosine", exact=True)

@@ -15,9 +15,10 @@
 namespace tpq {
 
 // ----------------------------------------------------------------------------- assignment: argmax_j sim(x_i, c_j)
-// data [l, d, n], cent [l, d, k]; sim = sum_e -(x-c)^2 (euclidean, fmaf(-dif, dif, acc), e ascending) or sum_e x*c.
+// data [l, d, n], cent [l, d, k]; sim = sum_e -(x-c)^2 (euclidean, fmaf(-dif, dif, acc), e ascending), sum_e x*c
+// (cosine, fmaf(x, c, acc)) or sum_e -|x-c| (manhattan, acc -= fabsf(x - c), max_sim.cu:100-120).
 constexpr int MS_B = 128, MS_K = 8;
-template <bool EUC>
+template <int METRIC>
 __global__ void __launch_bounds__(256)
 max_sim_kernel(const float* __restrict__ data, const float* __restrict__ cent, int d, int n, int k,
                float* __restrict__ maxsims, int64_t* __restrict__ labels) {
@@ -58,7 +59,8 @@ max_sim_kernel(const float* __restrict__ data, const float* __restrict__ cent, i
         for (int i = 0; i < 8; ++i)
           #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            if (EUC) { const float dif = a[i] - b[j]; acc[i][j] = fmaf(-dif, dif, acc[i][j]); }
+            if (METRIC == TPQ_METRIC_EUCLIDEAN) { const float dif = a[i] - b[j]; acc[i][j] = fmaf(-dif, dif, acc[i][j]); }
+            else if (METRIC == TPQ_METRIC_MANHATTAN) acc[i][j] -= fabsf(a[i] - b[j]);
             else acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
           }
       }
@@ -359,6 +361,24 @@ namespace tpq {
 bool assign_tc_supported(int l, int d, long long n, int k, const void* data, const void* cent);
 int launch_assign_tc(const float* data, const float* cent, int l, int d, long long n, int k, int exact_values,
                      float* maxsims, int64_t* labels, cudaStream_t st);
+bool assign_wide_supported(int l, int d, long long n, int k, const void* data, const void* cent);
+size_t assign_wide_workspace_bytes(int l, int d, int k);
+int launch_assign_wide(const float* data, const float* cent, int l, int d, long long n, int k, int metric,
+                       int exact_values, float* maxsims, int64_t* labels, void* ws, cudaStream_t st);
+
+// the exact SIMT kernel for one metric
+static int launch_max_sim_exact(const float* data, const float* centroids, int l, int d, int64_t n, int k, int metric,
+                                float* maxsims, int64_t* labels, cudaStream_t st) {
+  dim3 grid((unsigned)((n + MS_B - 1) / MS_B), l);
+  if (metric == TPQ_METRIC_EUCLIDEAN)
+    max_sim_kernel<TPQ_METRIC_EUCLIDEAN><<<grid, 256, 0, st>>>(data, centroids, d, (int)n, k, maxsims, labels);
+  else if (metric == TPQ_METRIC_MANHATTAN)
+    max_sim_kernel<TPQ_METRIC_MANHATTAN><<<grid, 256, 0, st>>>(data, centroids, d, (int)n, k, maxsims, labels);
+  else
+    max_sim_kernel<TPQ_METRIC_COSINE><<<grid, 256, 0, st>>>(data, centroids, d, (int)n, k, maxsims, labels);
+  TPQ_LAUNCH_CHECK("max_sim_kernel");
+  return TPQ_OK;
+}
 }
 
 using namespace tpq;
@@ -368,17 +388,40 @@ extern "C" int tpq_max_sim(const float* data, const float* centroids, int l, int
   TPQ_REQUIRE(data && centroids && maxsims && labels, "tpq_max_sim: null pointer");
   TPQ_REQUIRE(l > 0 && d > 0 && n >= 0 && k > 0, "tpq_max_sim: bad sizes l=%d d=%d n=%lld k=%d", l, d, (long long)n, k);
   TPQ_REQUIRE(n <= 0x7fffffffll - MS_B && l <= 65535, "tpq_max_sim: n or l too large");
-  TPQ_REQUIRE(metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE, "tpq_max_sim: unsupported metric %d", metric);
+  TPQ_REQUIRE(metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE || metric == TPQ_METRIC_MANHATTAN,
+              "tpq_max_sim: unsupported metric %d", metric);
   if (n == 0) return TPQ_OK;
   if (exact != 1 && metric == TPQ_METRIC_EUCLIDEAN && assign_tc_supported(l, d, n, k, data, centroids))
     return launch_assign_tc(data, centroids, l, d, n, k, exact == 2 ? 1 : 0, maxsims, labels, (cudaStream_t)stream);
-  dim3 grid((unsigned)((n + MS_B - 1) / MS_B), l);
-  if (metric == TPQ_METRIC_EUCLIDEAN)
-    max_sim_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(data, centroids, d, (int)n, k, maxsims, labels);
-  else
-    max_sim_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(data, centroids, d, (int)n, k, maxsims, labels);
-  TPQ_LAUNCH_CHECK("max_sim_kernel");
-  return TPQ_OK;
+  return launch_max_sim_exact(data, centroids, l, d, n, k, metric, maxsims, labels, (cudaStream_t)stream);
+}
+
+extern "C" size_t tpq_kmeans_assign_workspace_bytes(int l, int d, int k) {
+  return l > 0 && l <= 65535 ? assign_wide_workspace_bytes(l, d, k) : 0;
+}
+
+extern "C" int tpq_kmeans_assign(const float* data, const float* centroids, int l, int d, int64_t n, int k, int metric,
+                                 int exact_values, float* maxsims, int64_t* labels, void* ws, size_t ws_bytes,
+                                 void* stream) {
+  TPQ_REQUIRE(data && centroids && maxsims && labels, "tpq_kmeans_assign: null pointer");
+  TPQ_REQUIRE(l > 0 && d > 0 && n >= 0 && k > 0, "tpq_kmeans_assign: bad sizes l=%d d=%d n=%lld k=%d", l, d, (long long)n, k);
+  TPQ_REQUIRE(n <= 0x7fffffffll - MS_B && l <= 65535, "tpq_kmeans_assign: n or l too large");
+  TPQ_REQUIRE(metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE || metric == TPQ_METRIC_MANHATTAN,
+              "tpq_kmeans_assign: unsupported metric %d", metric);
+  if (n == 0) return TPQ_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ev = exact_values ? 1 : 0;
+  if (metric == TPQ_METRIC_EUCLIDEAN && assign_tc_supported(l, d, n, k, data, centroids))
+    return launch_assign_tc(data, centroids, l, d, n, k, ev, maxsims, labels, st);
+  if (metric != TPQ_METRIC_MANHATTAN && assign_wide_supported(l, d, n, k, data, centroids)) {
+    const size_t need = assign_wide_workspace_bytes(l, d, k);
+    if (!ws || ws_bytes < need || (reinterpret_cast<uintptr_t>(ws) & 15) != 0) {
+      set_error("tpq_kmeans_assign: workspace of %zu bytes at %p, need %zu bytes, 16-byte aligned", ws_bytes, ws, need);
+      return TPQ_ERR_WORKSPACE;
+    }
+    return launch_assign_wide(data, centroids, l, d, n, k, metric, ev, maxsims, labels, ws, st);
+  }
+  return launch_max_sim_exact(data, centroids, l, d, n, k, metric, maxsims, labels, st);
 }
 
 // Both kernels keep their sums on chip: no workspace (the ABI keeps the argument).

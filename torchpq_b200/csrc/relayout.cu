@@ -198,6 +198,7 @@ extern "C" int tpq_relayout_codebook(const float* pq_codebook, int d, int M, int
                                      float* pq_codebook_t, float* pq_norm_t, void* stream) {
   TPQ_REQUIRE(pq_codebook && pq_codebook_t && pq_norm_t, "tpq_relayout_codebook: null pointer");
   TPQ_REQUIRE(d > 0 && M > 0 && d % M == 0, "d_vector=%d must be a multiple of n_subvectors=%d", d, M);
+  TPQ_REQUIRE(metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE, "tpq_relayout_codebook: unsupported metric %d", metric);
   const int MP = (M + 31) / 32 * 32;
   int n = 256 * MP;
   relayout_codebook_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(pq_codebook, M, MP, d / M, metric,

@@ -94,7 +94,7 @@ class IVFPQTopk:
 
 def max_sim(data, centroids, distance="euclidean", exact=True, exact_values=True):
     """MultiKMeans.get_labels / MaxSimCuda(dim=2): data [l, d, n], centroids [l, d, k] ->
-    (maxsims [l, n] f32, labels [l, n] i64).  exact=False lets the TF32 tensor-core kernel run where it applies;
+    (maxsims [l, n] f32, labels [l, n] i64); distance "euclidean", "cosine" (inner product) or "manhattan".  exact=False lets the TF32 tensor-core kernel run where it applies;
     exact_values then selects exact fp32 maxsims for the chosen centroid (True) or TF32-derived ones (False, faster)."""
     a, b = _cuda_f32(data, "data"), _cuda_f32(centroids, "centroids")
     assert a.dim() == 3 and b.dim() == 3 and a.shape[:2] == b.shape[:2]
@@ -104,6 +104,24 @@ def max_sim(data, centroids, distance="euclidean", exact=True, exact_values=True
     labels = torch.empty(l, n, dtype=torch.long, device=a.device)
     check(lib.tpq_max_sim(ptr(a), ptr(b), l, d, n, k, _lib.METRIC[distance], 1 if exact else (2 if exact_values else 0), ptr(sims), ptr(labels),
                           _lib.current_stream(a.device)))
+    return sims, labels
+
+
+def kmeans_assign(data, centroids, distance="euclidean", exact_values=True):
+    """The assignment step of KMeans / MultiKMeans: data [l, d, n], centroids [l, d, k] -> (maxsims [l, n] f32,
+    labels [l, n] i64), on the TF32 tensor-core kernels wherever one takes the shape (tpq_kmeans_assign in
+    include/tpq_b200.h lists the ranges), else on the exact kernel.  distance "cosine" scores inner products: pass
+    normalised columns.  exact_values: exact fp32 maxsims for the chosen centroid (True) or TF32-derived ones."""
+    a, b = _cuda_f32(data, "data"), _cuda_f32(centroids, "centroids")
+    assert a.dim() == 3 and b.dim() == 3 and a.shape[:2] == b.shape[:2]
+    l, d, n = a.shape
+    k = b.shape[2]
+    sims = torch.empty(l, n, dtype=torch.float32, device=a.device)
+    labels = torch.empty(l, n, dtype=torch.long, device=a.device)
+    ws_bytes = lib.tpq_kmeans_assign_workspace_bytes(l, d, k)
+    ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=a.device)
+    check(lib.tpq_kmeans_assign(ptr(a), ptr(b), l, d, n, k, _lib.METRIC[distance], int(bool(exact_values)),
+                                ptr(sims), ptr(labels), ptr(ws), ws_bytes, _lib.current_stream(a.device)))
     return sims, labels
 
 
