@@ -54,7 +54,7 @@ typedef struct tpq_index {
   int32_t m_pad;                /* M rounded up to a multiple of 32 */
   int32_t shard_rank;           /* this shard owns cells c with c % shard_world == shard_rank */
   int32_t shard_world;
-  int32_t reserved0;
+  int32_t mean_cell_live;       /* live vectors per cell of this shard, rounded down (0 = unknown); selects the scan */
   int64_t n_blocks;             /* 32-vector blocks in codes_scan */
   const uint8_t*  codes_scan;   /* [n_blocks, m_pad/16, 32 lanes, 16 B], lane-rotated (DESIGN.md) */
   const uint32_t* block_valid;  /* [n_blocks] bit l set = vector l of the block is live */

@@ -31,7 +31,7 @@ class TpqIndex(C.Structure):
         ("vq_codebook", C.c_void_p), ("pq_codebook", C.c_void_p), ("storage", C.c_void_p),
         ("is_empty", C.c_void_p), ("cell_start", C.c_void_p), ("cell_size", C.c_void_p),
         ("address2id", C.c_void_p),
-        ("m_pad", C.c_int32), ("shard_rank", C.c_int32), ("shard_world", C.c_int32), ("reserved0", C.c_int32),
+        ("m_pad", C.c_int32), ("shard_rank", C.c_int32), ("shard_world", C.c_int32), ("mean_cell_live", C.c_int32),
         ("n_blocks", C.c_int64),
         ("codes_scan", C.c_void_p), ("block_valid", C.c_void_p), ("cell_block_start", C.c_void_p),
         ("pq_codebook_t", C.c_void_p), ("pq_norm_t", C.c_void_p),

@@ -200,8 +200,12 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
                               ptr(lay.codes_scan) if in_sync else None, ptr(lay.block_valid) if in_sync else None,
                               _lib.current_stream(dev)))
     index._max_id = max(index._max_id, int(ids.max().item()))
-    if not in_sync:                                                  # (in sync: the layout received the same items and stays valid;
-        index._state_changed()                                       #  raw-pointer writes do not move the buffers' fingerprint)
+    if in_sync:                                                      # the layout received the same items and stays valid
+        rank, world = lay.shard                                      # (raw-pointer writes do not move the buffers' fingerprint);
+        owned = n if world == 1 else int((cells % world == rank).sum().item())   # only the shard's cells reach block_valid
+        lay.set_live(lay.n_live + owned)
+    else:
+        index._state_changed()
     return (ids, write) if return_address else ids
 
 

@@ -28,6 +28,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace tpq {
 
@@ -276,6 +277,8 @@ struct ScanArgs {
   int nq, q_base, n_probe, k, kp, S;
   int boot_r;                     // blocks per warp in the bootstrap (1 or 2)
   int n_cells;                    // probe entries outside [0, n_cells) are treated as empty segments
+  const int* only_cnt;            // non-null: scan only the chunk's queries qi with only_cnt[qi] > only_cap (cell-major overflow)
+  int only_cap;
 #ifdef TPQ_DEBUG_KNOBS
   unsigned long long* phase;      // [8] summed clock64 deltas: prologue, bootstrap, scan, drain; [4] = CTAs
   int boot_mode;                  // 1 = merge-tree bootstrap (A/B against the quick start)
@@ -300,6 +303,52 @@ __device__ __forceinline__ void write_keys(const ScanArgs& A, const uint64_t* li
   for (int i = tid; i < A.k; i += NW * 32) out[i] = list[i];
 }
 
+// The LUT of query q in scan layout (RES: the query half of the residual LUT), built by the NW warps of a CTA
+// (PQCodec.py:62-75; MultiKMeans.py:183-223; same arithmetic as lut.cu).  Lane l owns sub-quantizers m = 32 h + l: reads
+// of the transposed codebook are contiguous across the warp, and so is every store (128 B), in shared or global memory.
+template <int MP, int NW, int DSUB, bool RES>
+__device__ __forceinline__ void build_lut(float* lutf, const float* __restrict__ x, const float* __restrict__ cbt, int M,
+                                          int nq, int q, int metric, int lane, int warp) {
+  constexpr int NH = MP / 32;
+  float xr[NH][DSUB], a2[NH];
+  #pragma unroll
+  for (int h = 0; h < NH; ++h) {
+    const int m = 32 * h + lane;
+    float s2 = 0.f;
+    #pragma unroll
+    for (int i = 0; i < DSUB; ++i) {
+      const float v = (m < M) ? __ldg(x + (size_t)(m * DSUB + i) * nq + q) : 0.f;
+      xr[h][i] = v;
+      s2 = __fadd_rn(s2, __fmul_rn(v, v));
+    }
+    a2[h] = s2;
+  }
+  #pragma unroll (DSUB >= 8 ? 2 : 8)
+  for (int c = warp; c < 256; c += NW) {
+    #pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const float* p = cbt + ((size_t)c * MP + 32 * h + lane) * DSUB;
+      float pv[DSUB];
+      if constexpr (DSUB == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); pv[0] = t.x; pv[1] = t.y; }
+      else if constexpr (DSUB % 4 == 0) {
+        #pragma unroll
+        for (int i = 0; i < DSUB; i += 4) {
+          const float4 t = __ldg(reinterpret_cast<const float4*>(p + i));
+          pv[i] = t.x; pv[i + 1] = t.y; pv[i + 2] = t.z; pv[i + 3] = t.w;
+        }
+      }
+      else { for (int i = 0; i < DSUB; ++i) pv[i] = __ldg(p + i); }
+      float dot = 0.f, b2 = 0.f;
+      #pragma unroll
+      for (int i = 0; i < DSUB; ++i) { dot = fmaf(xr[h][i], pv[i], dot); b2 = __fadd_rn(b2, __fmul_rn(pv[i], pv[i])); }
+      float y = dot;
+      if constexpr (RES) y = __fmul_rn(dot, 2.f);                    // part1 = 2 <x_m, p> (IVFPQIndex.py:377)
+      else if (metric == TPQ_METRIC_EUCLIDEAN) y = __fsub_rn(__fsub_rn(__fmul_rn(dot, 2.f), a2[h]), b2);
+      lutf[(h >> 1) * 16384 + c * 64 + (h & 1) * 32 + lane] = y;
+    }
+  }
+}
+
 // DSUB > 0: the CTA builds its query's LUT itself from the (L2-resident) transposed codebook -- no LUT
 // round trip through HBM, no LUT workspace.  DSUB == 0: the LUT was written by lut_scan_kernel and is copied in.
 // RES: residual IVFPQ (ivfpq_topk_residual_precomputed, ivfpq_topk.cu:1039-1207).  The LUT of a (query, cell) pair
@@ -318,6 +367,7 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
 
   const int qi = blockIdx.x / A.S, slice = blockIdx.x % A.S;  // query within this chunk
   const int q = A.q_base + qi;
+  if (A.only_cnt && A.only_cnt[qi] <= A.only_cap) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 #ifdef TPQ_DEBUG_KNOBS
   long long t_ph = clock64();
@@ -370,48 +420,9 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
     #pragma unroll 4
     for (int i = tid; i < MG * 4096; i += NW * 32) dst[i] = __ldg(src + i);
   } else {
-    // --- build the LUT in place (PQCodec.py:62-75; MultiKMeans.py:183-223; same arithmetic as lut.cu).
-    // Lane l owns sub-quantizers m = 32 h + l: reads of the transposed codebook are contiguous across the
-    // warp and the store bank is l, so both sides are conflict-free / coalesced.
-    constexpr int NH = MP / 32;
-    float xr[NH][DSUB], a2[NH];
-    #pragma unroll
-    for (int h = 0; h < NH; ++h) {
-      const int m = 32 * h + lane;
-      float s2 = 0.f;
-      #pragma unroll
-      for (int i = 0; i < DSUB; ++i) {
-        const float v = (m < A.M) ? __ldg(A.x + (size_t)(m * DSUB + i) * A.nq + q) : 0.f;
-        xr[h][i] = v;
-        s2 = __fadd_rn(s2, __fmul_rn(v, v));
-      }
-      a2[h] = s2;
-    }
-    float* lutf = reinterpret_cast<float*>(RES ? smem + L.part1 : lut);
-    #pragma unroll (DSUB >= 8 ? 2 : 8)
-    for (int c = warp; c < 256; c += NW) {
-      #pragma unroll
-      for (int h = 0; h < NH; ++h) {
-        const float* p = A.cbt + ((size_t)c * MP + 32 * h + lane) * DSUB;
-        float pv[DSUB];
-        if constexpr (DSUB == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); pv[0] = t.x; pv[1] = t.y; }
-        else if constexpr (DSUB % 4 == 0) {
-          #pragma unroll
-          for (int i = 0; i < DSUB; i += 4) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(p + i));
-            pv[i] = t.x; pv[i + 1] = t.y; pv[i + 2] = t.z; pv[i + 3] = t.w;
-          }
-        }
-        else { for (int i = 0; i < DSUB; ++i) pv[i] = __ldg(p + i); }
-        float dot = 0.f, b2 = 0.f;
-        #pragma unroll
-        for (int i = 0; i < DSUB; ++i) { dot = fmaf(xr[h][i], pv[i], dot); b2 = __fadd_rn(b2, __fmul_rn(pv[i], pv[i])); }
-        float y = dot;
-        if constexpr (RES) y = __fmul_rn(dot, 2.f);                    // part1 = 2 <x_m, p> (IVFPQIndex.py:377)
-        else if (A.metric == TPQ_METRIC_EUCLIDEAN) y = __fsub_rn(__fsub_rn(__fmul_rn(dot, 2.f), a2[h]), b2);
-        lutf[(h >> 1) * 16384 + c * 64 + (h & 1) * 32 + lane] = y;
-      }
-    }
+    // --- build the LUT in place (or, RES, the query half of the residual LUT)
+    build_lut<MP, NW, DSUB, RES>(reinterpret_cast<float*>(RES ? smem + L.part1 : lut), A.x, A.cbt, A.M, A.nq, q, A.metric,
+                                 lane, warp);
   }
 #ifdef TPQ_DEBUG_KNOBS
   auto phase_mark = [&](int i) {
@@ -547,6 +558,284 @@ static int launch_merge(const uint64_t* keys_in, int nq, int n_parts, int k, int
   return TPQ_OK;
 }
 
+// ----------------------------------------------------------------------------- cell-major scan (M <= 64, large cells)
+// The query-major kernel reads a probed cell's codes once per (query, cell) pair: at 2441 vectors per cell that is
+// 156 KB per pair against a 64 KB LUT.  The cell-major path turns the loop around: a CTA holds a chunk of one cell's
+// code blocks in registers and the LUTs of the queries probing that cell stream past it, so a pair costs one LUT read.
+//   pass 1  the query-major kernel on each query's first probe entry -> its sorted top-k; key k-1 bounds the query
+//           (0 when that cell has fewer than k live vectors);
+//   pass 2  ivfpq_cell_scan_kernel over entries 1 .. P-1: every key above the bound is appended to the query's survivors;
+//   select  per query, the top k of the pass-1 list and the survivors (cell_select_kernel).
+// Exact: a candidate that is neither in the pass-1 list nor a survivor is <= the bound, and the pass-1 list already
+// holds k keys >= the bound.  Scores are formed exactly as in the query-major kernel, so results are bit-identical.
+constexpr int kCellSlots = 3;         // LUT ring depth (64 KB each)
+constexpr int kCellNW = 12;           // warps of a cell-scan CTA
+constexpr int kCellR = 7;             // code blocks per warp held in registers (168 registers): a chunk is up to 84 blocks = 2688 vectors
+constexpr int kCellChunk = kCellNW * kCellR;
+constexpr int kCellBuckets = 128;     // work classes of the largest-first item order (4 per octave)
+
+struct CellItem { int32_t cell, b_lo, b_hi, pad; };   // blocks [b_lo, b_hi) of the cell (relative to its first block)
+
+struct CellArgs {
+  const uint8_t* codes; const uint32_t* valid; const int32_t* cell_block_start; const int64_t* cell_start;
+  const float* lut_scan;          // [n][256][64] LUTs of this chunk's queries (cell_lut_kernel)
+  const int32_t* cell_off;        // [C] first pair of each cell in pair_q
+  const int32_t* cell_cnt;        // [C] pairs per cell
+  const int32_t* pair_q;          // chunk-local query of each pair, grouped by cell
+  const CellItem* items; const int* n_items; int* cursor;
+  const uint64_t* keys;           // [nq][k] pass-1 lists; key k-1 is the query's bound
+  uint64_t* surv; int* surv_cnt;  // [n][cap] survivors, [n] their count (> cap: overflow), by chunk-local query
+  int q_base, k, cap;
+};
+
+// the cell of probe entry j >= 1 of query row cq if the query-major kernel scans it (same rules as its prologue), else -1
+__device__ __forceinline__ int64_t visited_cell(const int64_t* cq, int j, int n_cells, const int64_t* cell_start,
+                                                const int64_t* cell_size, const int32_t* cbs) {
+  const int64_t c = cq[j];
+  if (c < 0 || c >= n_cells) return -1;
+  const int64_t cp = cq[j - 1];
+  if (cp >= 0 && cp < n_cells && cell_start[c] == cell_start[cp]) return -1;
+  const int64_t sz = cell_size[c];
+  const int64_t nb = min((int64_t)(cbs[c + 1] - cbs[c]), sz > 0 ? (sz + 31) >> 5 : (int64_t)0);
+  return nb > 0 ? c : -1;
+}
+
+// thread per (query, entry): count the visited pairs of entries 1 .. P-1 per cell; slot = the pair's rank in its cell
+__global__ void cell_pairs_count_kernel(const int64_t* __restrict__ cells, const int64_t* __restrict__ npl, int q_base, int n,
+                                        int n_probe, int n_cells, const int64_t* __restrict__ cell_start,
+                                        const int64_t* __restrict__ cell_size, const int32_t* __restrict__ cbs,
+                                        int* __restrict__ cell_cnt, int* __restrict__ slot, int64_t* __restrict__ ones) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)n * n_probe) return;
+  const int qi = (int)(t / n_probe), j = (int)(t % n_probe);
+  const int q = q_base + qi;
+  if (j == 0) ones[q] = 1;                                     // pass 1 scans entry 0 only
+  int P = (int)npl[q];
+  P = max(1, min(P, n_probe));
+  int pos = -1;
+  if (j >= 1 && j < P) {
+    const int64_t c = visited_cell(cells + (size_t)q * n_probe, j, n_cells, cell_start, cell_size, cbs);
+    if (c >= 0) pos = atomicAdd(cell_cnt + c, 1);
+  }
+  slot[t] = pos;
+}
+
+__global__ void cell_pairs_scatter_kernel(const int64_t* __restrict__ cells, int q_base, int n, int n_probe,
+                                          const int* __restrict__ slot, const int* __restrict__ cell_off,
+                                          int* __restrict__ pair_q) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)n * n_probe) return;
+  const int s = slot[t];
+  if (s < 0) return;
+  const int qi = (int)(t / n_probe);
+  pair_q[cell_off[cells[(size_t)(q_base + qi) * n_probe + t % n_probe]] + s] = qi;
+}
+
+// One CTA: cell_off = exclusive prefix of cell_cnt; work items = chunks of at most kCellChunk blocks of every cell with
+// pairs, ordered by work (pairs x blocks) descending in classes of 4 per octave, the chunks of one cell adjacent.
+__global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__ cell_cnt, const int32_t* __restrict__ cbs,
+                                                         const int64_t* __restrict__ cell_size, int n_cells,
+                                                         int* __restrict__ cell_off, CellItem* __restrict__ items,
+                                                         int* __restrict__ n_items) {
+  __shared__ int hist[kCellBuckets], base[kCellBuckets], warp_sum[32], carry;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = tid; i < kCellBuckets; i += 1024) hist[i] = 0;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  auto chunks_of = [&](int c, int& nb, int& bucket) {
+    const int64_t sz = cell_size[c];
+    nb = (int)min((int64_t)(cbs[c + 1] - cbs[c]), sz > 0 ? (sz + 31) >> 5 : (int64_t)0);
+    const int np = cell_cnt[c];
+    if (np == 0 || nb == 0) { nb = 0; return 0; }
+    const int nch = (nb + kCellChunk - 1) / kCellChunk;
+    const uint32_t w = (uint32_t)np * (uint32_t)((nb + nch - 1) / nch);
+    const int lg = 31 - __clz(w);
+    const int sub = lg >= 2 ? (int)((w >> (lg - 2)) & 3u) : (int)((w << (2 - lg)) & 3u);
+    bucket = kCellBuckets - 1 - min(kCellBuckets - 1, 4 * lg + sub);   // larger work -> smaller bucket index
+    return nch;
+  };
+  for (int c0 = 0; c0 < n_cells; c0 += 1024) {
+    const int c = c0 + tid;
+    const int v = c < n_cells ? cell_cnt[c] : 0;
+    int incl = v;
+    #pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += y; }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+      int s = warp_sum[lane], si = s;
+      #pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, si, o); if (lane >= o) si += y; }
+      warp_sum[lane] = si - s;
+    }
+    __syncthreads();
+    if (c < n_cells) {
+      cell_off[c] = carry + warp_sum[warp] + incl - v;
+      int nb, b;
+      const int nch = chunks_of(c, nb, b);
+      if (nch) atomicAdd(&hist[b], nch);
+    }
+    __syncthreads();
+    if (tid == 1023) carry += warp_sum[31] + incl;
+    __syncthreads();
+  }
+  if (tid == 0) {
+    int s = 0;
+    for (int b = 0; b < kCellBuckets; ++b) { base[b] = s; s += hist[b]; }
+    *n_items = s;
+  }
+  __syncthreads();
+  for (int c = tid; c < n_cells; c += 1024) {
+    int nb, b;
+    const int nch = chunks_of(c, nb, b);
+    if (!nch) continue;
+    const int pos = atomicAdd(&base[b], nch);
+    for (int j = 0; j < nch; ++j)
+      items[pos + j] = CellItem{c, (int)((int64_t)nb * j / nch), (int)((int64_t)nb * (j + 1) / nch), 0};
+  }
+}
+
+// Persistent: a CTA takes items (cell, chunk) from a global cursor.  Warp w holds blocks w, w + NW, ... of the chunk
+// (R at most) in registers.  The LUTs of the pairs of the cell arrive by TMA into a ring of kCellSlots 64 KB slots; the
+// last warp to finish with a slot refills it, so no warp waits for another except through the ring.  Per block the
+// scoring is the query-major kernel's adc_unit, so a key is the same bit for bit.
+template <int NW, int R>
+__global__ void __launch_bounds__(NW * 32, 1)
+ivfpq_cell_scan_kernel(CellArgs A) {
+  constexpr int MP = 64;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* ring = smem;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kCellSlots * 65536);
+  uint64_t* slot_thr = full + kCellSlots;
+  int* slot_q = reinterpret_cast<int*>(slot_thr + kCellSlots);
+  int* rel = slot_q + kCellSlots;                              // warps done with the slot's current LUT
+  int* item_sh = rel + kCellSlots;                             // [2]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  uint64_t* stage = reinterpret_cast<uint64_t*>(smem + kCellSlots * 65536 + 256) + (size_t)warp * R * 32;
+  if (tid == 0) {
+    for (int s = 0; s < kCellSlots; ++s) { mbar_init(&full[s], 1); rel[s] = 0; }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  uint32_t off[8];
+  #pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    uint32_t v = 0;
+    #pragma unroll
+    for (int b = 0; b < 4; ++b) v |= (uint32_t)(((lane + 4 * i + b) & 31) * 4) << (8 * b);
+    off[i] = v;
+  }
+  // one thread: LUT of pair i of the current cell into slot s (every warp has released the slot)
+  auto issue = [&](const int32_t* pq, int i, int s) {
+    const int qi = pq[i];
+    slot_q[s] = qi;
+    slot_thr[s] = A.keys[(size_t)(A.q_base + qi) * A.k + A.k - 1];
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the warps' reads of the slot precede the TMA write
+    mbar_expect_tx(&full[s], 65536);
+    bulk_load(ring + s * 65536, A.lut_scan + (size_t)qi * 16384, 65536, &full[s]);
+  };
+  uint32_t seq = 0;                                            // LUTs consumed by this CTA so far
+  const int n_items = *A.n_items;
+  for (int it = 0;; ++it) {
+    if (tid == 0) item_sh[it & 1] = atomicAdd(A.cursor, 1);
+    __syncthreads();                                           // also: every warp is done with the previous item
+    const int item = item_sh[it & 1];
+    if (item >= n_items) break;
+    const CellItem ci = A.items[item];
+    const int np = A.cell_cnt[ci.cell];
+    const int32_t* pq = A.pair_q + A.cell_off[ci.cell];
+    if (tid == 0)
+      for (int i = 0; i < min(np, kCellSlots); ++i) issue(pq, i, (seq + i) % kCellSlots);
+    const int b0 = A.cell_block_start[ci.cell];
+    const uint32_t a0 = (uint32_t)A.cell_start[ci.cell];
+    const int nr = (ci.b_hi - ci.b_lo - warp + NW - 1) / NW;   // blocks of this warp (may be <= 0)
+    uint32_t w[R][16], vmask[R];
+    #pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (r < nr) {
+        const int64_t B = (int64_t)b0 + ci.b_lo + warp + r * NW;
+        load_unit<MP, 0>(w[r], A.codes, B, lane);
+        vmask[r] = __ldg(A.valid + B);
+      }
+    }
+    for (int i = 0; i < np; ++i, ++seq) {
+      const int s = seq % kCellSlots;
+      mbar_wait(&full[s], (seq / kCellSlots) & 1);
+      const int qi = slot_q[s];
+      const uint64_t thr = slot_thr[s];
+      const uint8_t* lut = ring + s * 65536;
+      int n = 0;
+      #pragma unroll
+      for (int r = 0; r < R; ++r) {
+        if (r < nr) {
+          float acc[4] = {0.f, 0.f, 0.f, 0.f};
+          adc_unit<MP, 0>(w[r], off, lut, acc);
+          const float score = (acc[0] + acc[1]) + (acc[2] + acc[3]);
+          const uint64_t key = make_key(score, a0 + (uint32_t)(ci.b_lo + warp + r * NW) * 32u + lane);
+          const bool pass = ((vmask[r] >> lane) & 1u) && key > thr;
+          const unsigned m = __ballot_sync(0xffffffffu, pass);
+          if (pass) stage[n + __popc(m & ((1u << lane) - 1))] = key;
+          n += __popc(m);
+        }
+      }
+      __syncwarp();
+      if (lane == 0) {                                         // release the slot; the last warp refills it
+        int old;
+        asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(smem_u32(&rel[s])) : "memory");
+        if (old == NW - 1) {
+          rel[s] = 0;
+          if (i + kCellSlots < np) issue(pq, i + kCellSlots, s);
+        }
+      }
+      if (n) {
+        int base = 0;
+        if (lane == 0) base = atomicAdd(A.surv_cnt + qi, n);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (base + n <= A.cap) {
+          uint64_t* dst = A.surv + (size_t)qi * A.cap + base;
+          for (int j = lane; j < n; j += 32) dst[j] = stage[j];
+        }
+        __syncwarp();
+      }
+    }
+  }
+}
+
+// CTA per query: its LUT in scan layout into global memory, as the query-major kernel builds it in shared memory
+template <int DSUB>
+__global__ void __launch_bounds__(256) cell_lut_kernel(const float* __restrict__ x, const float* __restrict__ cbt, int M,
+                                                       int nq, int q_base, int metric, float* __restrict__ lut) {
+  build_lut<64, 8, DSUB, false>(lut + (size_t)blockIdx.x * 16384, x, cbt, M, nq, q_base + blockIdx.x, metric,
+                                threadIdx.x & 31, threadIdx.x >> 5);
+}
+
+// warp per query: keys[q] <- top k of keys[q] (the pass-1 list) and the survivors; overflowed queries are left to the
+// query-major re-run
+__global__ void __launch_bounds__(128) cell_select_kernel(uint64_t* __restrict__ keys, const uint64_t* __restrict__ surv,
+                                                          const int* __restrict__ surv_cnt, int q_base, int n, int k,
+                                                          int kp, int cap) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int qi = blockIdx.x * 4 + warp;
+  if (qi >= n) return;
+  const int q = q_base + qi;
+  const int ns = surv_cnt[qi];
+  if (ns == 0 || ns > cap) return;
+  uint64_t* list = reinterpret_cast<uint64_t*>(smem) + (size_t)warp * (kp + kTopkBuf);
+  WarpTopK tk;
+  tk.init(list, list + kp, kp, k, lane);
+  uint64_t* kq = keys + (size_t)q * k;
+  for (int i = lane; i < k; i += 32) list[i] = kq[i];
+  __syncwarp();
+  const uint64_t* sq = surv + (size_t)qi * cap;
+  for (int i0 = 0; i0 < ns; i0 += 32) {
+    const uint64_t key = i0 + lane < ns ? sq[i0 + lane] : 0ull;
+    tk.push(key > tk.kth(), key, lane);
+  }
+  tk.flush(lane);
+  __syncwarp();
+  for (int i = lane; i < k; i += 32) kq[i] = list[i];
+}
+
 // ----------------------------------------------------------------------------- host orchestration
 constexpr int kQueryChunk = 16384;    // queries per scan launch (bounds the LUT workspace: 64 KB * MG each)
 
@@ -589,23 +878,63 @@ static int fused_dsub(const tpq_index* ix) {
 
 struct PeerOut { uint64_t* keys[8]; int n, slot; };
 
+// Cell-major scan when a pair's LUT (64 KB) is clearly smaller than the codes of the cell it meets: the plain index at
+// M <= 64 whose cells hold more than kCellMinLive live vectors (codes) on average, on an unsliced batch.  Unsharded only:
+// on a cell shard, a query's entry 0 is usually another shard's cell, which gives pass 1 no vectors and the bound 0, so
+// every owned candidate would survive and overflow.
+constexpr int kCellMinLive = 1536;
+static bool cell_major(const tpq_index* ix, int S) {
+  return !ix->residual && ix->m_pad == 64 && fused_dsub(ix) && S == 1 && ix->shard_world == 1 && ix->n_blocks > 0 &&
+         ix->mean_cell_live >= kCellMinLive;
+}
+// survivors kept per query; a query with more is scanned again by the query-major kernel
+static int cell_cap(int k) { return k * 8 > 8192 ? k * 8 : 8192; }
+
 struct SearchWs {
-  size_t coarse, probe_sims, cells, npl, xnorm, lut, keys, total;
+  size_t coarse, probe_sims, cells, npl, xnorm, lut, keys;
+  size_t cell_cnt, cell_off, slot, pair_q, items, ones, surv, surv_cnt;   // cell-major scan only
+  size_t total;
 };
-static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k) {
+// push: the fused-push path (tpq_ivfpq_scan_push), which keeps the query-major kernel
+static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, bool push = false) {
   SearchWs w; size_t off = 0;
   const int MG = (ix->m_pad + 63) / 64;
   const int chunk = nq < kQueryChunk ? nq : kQueryChunk;
   const int S = pick_slices(ix, nq, k);
+  const bool cm = !push && cell_major(ix, S);
   w.coarse = off;     off += align_up(tpq_coarse_workspace_bytes(ix->d_vector, nq, ix->n_cells), 256);
   w.probe_sims = off; off += align_up((size_t)nq * n_probe * 4, 256);
   w.cells = off;      off += align_up((size_t)nq * n_probe * 8, 256);
   w.npl = off;        off += align_up((size_t)nq * 8, 256);
   w.xnorm = off;      off += align_up((size_t)nq * ix->d_vector * 4, 256);
-  w.lut = off;        off += fused_dsub(ix) ? 0 : align_up((size_t)chunk * MG * 65536, 256);
+  w.lut = off;        off += fused_dsub(ix) && !cm ? 0 : align_up((size_t)chunk * MG * 65536, 256);
   w.keys = off;       off += align_up((size_t)nq * S * k * 8, 256);
+  const size_t C = cm ? (size_t)ix->n_cells : 0, pairs = cm ? (size_t)chunk * n_probe : 0;
+  const size_t n_items = cm ? C + (size_t)ix->n_blocks / kCellChunk + 1 : 0;
+  w.cell_cnt = off;   off += align_up((C + 2) * 4, 256);                  // pairs per cell, then the item count and cursor
+  w.cell_off = off;   off += align_up(C * 4, 256);
+  w.slot = off;       off += align_up(pairs * 4, 256);
+  w.pair_q = off;     off += align_up(pairs * 4, 256);
+  w.items = off;      off += align_up(n_items * sizeof(CellItem), 256);
+  w.ones = off;       off += align_up(cm ? (size_t)nq * 8 : 0, 256);
+  w.surv = off;       off += align_up(cm ? (size_t)chunk * cell_cap(k) * 8 : 0, 256);
+  w.surv_cnt = off;   off += align_up(cm ? (size_t)chunk * 4 : 0, 256);
   w.total = off;
   return w;
+}
+
+static ScanArgs scan_args(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl, int nq, int q0,
+                          int n_probe, int k, int S, const float* lut_ws, uint64_t* keys, const float* base_sims) {
+  ScanArgs A;
+  A.x = x; A.cbt = ix->pq_codebook_t; A.M = ix->n_subvectors; A.metric = ix->metric;
+  A.part2_scan = ix->part2_scan; A.base_sims = base_sims;
+  A.codes = ix->codes_scan; A.valid = ix->block_valid; A.cell_block_start = ix->cell_block_start;
+  A.cell_start = ix->cell_start; A.cell_size = ix->cell_size; A.lut_scan = lut_ws; A.cells = cells; A.n_probe_list = npl; A.keys_out = keys;
+  A.nq = nq; A.q_base = q0; A.n_probe = n_probe; A.k = k; A.kp = next_pow2(k < 32 ? 32 : k); A.S = S;
+  A.boot_r = 2; A.n_cells = ix->n_cells;
+  A.n_peers = 0; A.peer_slot = 0;
+  A.only_cnt = nullptr; A.only_cap = 0;
+  return A;
 }
 
 template <int MP, int NW, int MINB, int DSUB, bool RES = false>
@@ -631,14 +960,7 @@ static int launch_scan_d(const tpq_index* ix, const float* x, const int64_t* cel
                                                     nq, q0, n, RES ? kLutPart1 : ix->metric, lut_ws);
       TPQ_LAUNCH_CHECK("lut_scan_kernel");
     }
-    ScanArgs A;
-    A.x = x; A.cbt = ix->pq_codebook_t; A.M = ix->n_subvectors; A.metric = ix->metric;
-    A.part2_scan = ix->part2_scan; A.base_sims = base_sims;
-    A.codes = ix->codes_scan; A.valid = ix->block_valid; A.cell_block_start = ix->cell_block_start;
-    A.cell_start = ix->cell_start; A.cell_size = ix->cell_size; A.lut_scan = lut_ws; A.cells = cells; A.n_probe_list = npl; A.keys_out = keys;
-    A.nq = nq; A.q_base = q0; A.n_probe = n_probe; A.k = k; A.kp = kp; A.S = S;
-    A.boot_r = 2; A.n_cells = ix->n_cells;
-    A.n_peers = 0; A.peer_slot = 0;
+    ScanArgs A = scan_args(ix, x, cells, npl, nq, q0, n_probe, k, S, lut_ws, keys, base_sims);
     if (peers) { A.n_peers = peers->n; A.peer_slot = peers->slot; for (int p = 0; p < peers->n; ++p) A.peer_keys[p] = peers->keys[p]; }
 #ifdef TPQ_DEBUG_KNOBS
     { const char* br = getenv("TPQ_BOOT_R"); if (br && atoi(br) == 1) A.boot_r = 1; }
@@ -667,6 +989,74 @@ static int launch_scan(const tpq_index* ix, const float* x, const int64_t* cells
   }
 }
 
+// The cell-major scan of a batch (see ivfpq_cell_scan_kernel), per chunk of kQueryChunk queries; leaves keys [nq][k].
+// The profiling events bracket the whole stage: LUTs, pass 1, pair list, pass 2, select and re-run.
+template <int DSUB>
+static int launch_cell_path(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl, int nq,
+                            int n_probe, int k, uint8_t* w, const SearchWs& W, uint64_t* keys, cudaStream_t st) {
+  const int kp = next_pow2(k < 32 ? 32 : k);
+  const int cap = cell_cap(k);
+  const int C = ix->n_cells;
+  float* lut_ws = reinterpret_cast<float*>(w + W.lut);
+  int* cell_cnt = reinterpret_cast<int*>(w + W.cell_cnt);
+  int* n_items = cell_cnt + C;
+  int* cell_off = reinterpret_cast<int*>(w + W.cell_off);
+  int* slot = reinterpret_cast<int*>(w + W.slot);
+  int* pair_q = reinterpret_cast<int*>(w + W.pair_q);
+  CellItem* items = reinterpret_cast<CellItem*>(w + W.items);
+  int64_t* ones = reinterpret_cast<int64_t*>(w + W.ones);
+  uint64_t* surv = reinterpret_cast<uint64_t*>(w + W.surv);
+  int* surv_cnt = reinterpret_cast<int*>(w + W.surv_cnt);
+
+  const ScanSmem L = scan_smem(64, n_probe, 8, kp);
+  if (L.total > 227 * 1024) {
+    set_error("scan: M=%d n_probe=%d k=%d needs %zu B of shared memory (> 227 KB)", ix->n_subvectors, n_probe, k, L.total);
+    return TPQ_ERR_UNSUPPORTED;
+  }
+  auto qmajor = ivfpq_scan_kernel<64, 8, 2, 0, false>;                  // 120 registers, 0 spill bytes
+  TPQ_CUDA(cudaFuncSetAttribute(qmajor, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
+  auto cscan = ivfpq_cell_scan_kernel<kCellNW, kCellR>;
+  const size_t cs_smem = (size_t)kCellSlots * 65536 + 256 + (size_t)kCellChunk * 32 * 8;
+  TPQ_CUDA(cudaFuncSetAttribute(cscan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
+  const size_t sel_smem = (size_t)4 * (kp + kTopkBuf) * 8;
+  TPQ_CUDA(cudaFuncSetAttribute(cell_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
+  for (int q0 = 0; q0 < nq; q0 += kQueryChunk) {
+    const int n = (nq - q0) < kQueryChunk ? (nq - q0) : kQueryChunk;
+    const bool prof = g_prof_on && g_prof_n < kProfMax;
+    if (prof) cudaEventRecord(g_prof_start[g_prof_n], st);
+    TPQ_CUDA(cudaMemsetAsync(cell_cnt, 0, (size_t)(C + 2) * 4, st));
+    TPQ_CUDA(cudaMemsetAsync(surv_cnt, 0, (size_t)n * 4, st));
+    cell_lut_kernel<DSUB><<<n, 256, 0, st>>>(x, ix->pq_codebook_t, ix->n_subvectors, nq, q0, ix->metric, lut_ws);
+    TPQ_LAUNCH_CHECK("cell_lut_kernel");
+    const int64_t nt = (int64_t)n * n_probe;
+    const int pgrid = (int)((nt + 255) / 256);
+    cell_pairs_count_kernel<<<pgrid, 256, 0, st>>>(cells, npl, q0, n, n_probe, C, ix->cell_start, ix->cell_size,
+                                                   ix->cell_block_start, cell_cnt, slot, ones);
+    TPQ_LAUNCH_CHECK("cell_pairs_count_kernel");
+    ScanArgs A = scan_args(ix, x, cells, ones, nq, q0, n_probe, k, 1, lut_ws, keys, nullptr);
+    qmajor<<<n, 8 * 32, L.total, st>>>(A, L);                              // pass 1: entry 0 of every query
+    TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
+    cell_plan_kernel<<<1, 1024, 0, st>>>(cell_cnt, ix->cell_block_start, ix->cell_size, C, cell_off, items, n_items);
+    TPQ_LAUNCH_CHECK("cell_plan_kernel");
+    cell_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(cells, q0, n, n_probe, slot, cell_off, pair_q);
+    TPQ_LAUNCH_CHECK("cell_pairs_scatter_kernel");
+    CellArgs CA;
+    CA.codes = ix->codes_scan; CA.valid = ix->block_valid; CA.cell_block_start = ix->cell_block_start;
+    CA.cell_start = ix->cell_start; CA.lut_scan = lut_ws; CA.cell_off = cell_off; CA.cell_cnt = cell_cnt; CA.pair_q = pair_q;
+    CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
+    CA.q_base = q0; CA.k = k; CA.cap = cap;
+    cscan<<<device_sm_count(), kCellNW * 32, cs_smem, st>>>(CA);
+    TPQ_LAUNCH_CHECK("ivfpq_cell_scan_kernel");
+    cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(keys, surv, surv_cnt, q0, n, k, kp, cap);
+    TPQ_LAUNCH_CHECK("cell_select_kernel");
+    A.n_probe_list = npl; A.only_cnt = surv_cnt; A.only_cap = cap;
+    qmajor<<<n, 8 * 32, L.total, st>>>(A, L);                              // queries whose survivors overflowed
+    TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
+    if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], st);
+  }
+  return TPQ_OK;
+}
+
 static int check_index(const tpq_index* ix) {
   TPQ_REQUIRE(ix, "null index");
   TPQ_REQUIRE(ix->d_vector > 0 && ix->n_subvectors > 0 && ix->d_vector % ix->n_subvectors == 0,
@@ -683,9 +1073,20 @@ static int check_index(const tpq_index* ix) {
   return TPQ_OK;
 }
 
+// ws/W: the search workspace, for the cell-major path (nullptr: the fused-push path, which keeps the query-major kernel)
 static int scan_dispatch(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl,
                          int nq, int n_probe, int k, int S, float* lut_ws, uint64_t* keys, cudaStream_t st,
-                         const float* base_sims = nullptr, const PeerOut* peers = nullptr) {
+                         const float* base_sims, uint8_t* ws, const SearchWs* W, const PeerOut* peers = nullptr) {
+  if (ws && !peers && cell_major(ix, S)) {
+#define TPQ_CELL(DS) launch_cell_path<DS>(ix, x, cells, npl, nq, n_probe, k, ws, *W, keys, st)
+    switch (fused_dsub(ix)) {
+      case 1:  return TPQ_CELL(1);
+      case 2:  return TPQ_CELL(2);
+      case 4:  return TPQ_CELL(4);
+      default: return TPQ_CELL(8);
+    }
+#undef TPQ_CELL
+  }
   if (ix->residual) {
     // residual IVFPQ.  M <= 64 and d/M in {1,2,4}: the query half of the LUT is built once into a second shared-memory
     // table (two 64 KB tables -> one 16-warp CTA per SM).  Otherwise (M up to 192, any d/M) the query half is staged in
@@ -802,7 +1203,7 @@ extern "C" int tpq_ivfpq_search_cells(const tpq_index* ix, const float* x_dn, co
   const int S = pick_slices(ix, nq, k);
   uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
   if (int rc = scan_dispatch(ix, x_dn, cells, n_probe_list, nq, n_probe, k, S,
-                             reinterpret_cast<float*>(w + W.lut), keys, st, base_sims)) return rc;
+                             reinterpret_cast<float*>(w + W.lut), keys, st, base_sims, w, &W)) return rc;
   return launch_merge(keys, nq, S, k, k, (int64_t)S * k, ix->address2id, ix->capacity, values, ids, address, keys_out, st);
 }
 
@@ -832,7 +1233,8 @@ extern "C" int tpq_ivfpq_search(const tpq_index* ix, const float* x_dn, int nq, 
   cudaStream_t st = (cudaStream_t)stream;
   const int S = pick_slices(ix, nq, k);
   uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
-  if (int rc = scan_dispatch(ix, x, cells, npl, nq, n_probe, k, S, reinterpret_cast<float*>(w + W.lut), keys, st, probe_sims)) return rc;
+  if (int rc = scan_dispatch(ix, x, cells, npl, nq, n_probe, k, S, reinterpret_cast<float*>(w + W.lut), keys, st, probe_sims,
+                             w, &W)) return rc;
   return launch_merge(keys, nq, S, k, k, (int64_t)S * k, ix->address2id, ix->capacity, values, ids, address, keys_out, st);
 }
 
@@ -848,7 +1250,7 @@ extern "C" int tpq_ivfpq_scan_push(const tpq_index* ix, const float* x_dn, const
   if (nq == 0) return TPQ_OK;
   if (pick_slices(ix, nq, k) != 1) { set_error("tpq_ivfpq_scan_push: batch of %d queries is sliced; use the gathered exchange", nq); return TPQ_ERR_UNSUPPORTED; }
   if (nq > kQueryChunk) { set_error("tpq_ivfpq_scan_push: at most %d queries per call", kQueryChunk); return TPQ_ERR_UNSUPPORTED; }
-  SearchWs W = search_ws(ix, nq, n_probe, k);
+  SearchWs W = search_ws(ix, nq, n_probe, k, /*push=*/true);
   if (!ws || ws_bytes < W.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, W.total); return TPQ_ERR_WORKSPACE; }
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
   const float* x = x_dn;
@@ -870,7 +1272,7 @@ extern "C" int tpq_ivfpq_scan_push(const tpq_index* ix, const float* x_dn, const
   po.n = n_peers; po.slot = my_slot;
   for (int p = 0; p < n_peers; ++p) { TPQ_REQUIRE(peer_keys[p], "null peer buffer"); po.keys[p] = peer_keys[p]; }
   return scan_dispatch(ix, x, cells, n_probe_list, nq, n_probe, k, 1, reinterpret_cast<float*>(w + W.lut),
-                       reinterpret_cast<uint64_t*>(w + W.keys), (cudaStream_t)stream, base_sims, &po);
+                       reinterpret_cast<uint64_t*>(w + W.keys), (cudaStream_t)stream, base_sims, nullptr, nullptr, &po);
 }
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k,

@@ -31,6 +31,11 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       :: "r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// contiguous global -> shared copy by the TMA unit (bytes % 16 == 0, both ends 16-byte aligned)
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
 
 // wgmma shared-memory matrix descriptor, K-major operand with the 128-byte swizzle: 8-row x 128-byte atoms, rows
 // 128 bytes apart, atoms SBO = 1024 bytes apart along N; LBO is unused for swizzled K-major layouts (encoded 1).

@@ -97,10 +97,20 @@ class ScanLayout:
         if parts is None:
             check(lib.tpq_relayout_codes(C.byref(ix), ptr(self.codes_scan), ptr(self.block_valid), stream))
         check(lib.tpq_relayout_codebook(ptr(pq), d, M, ix.metric, ptr(self.pq_codebook_t), ptr(self.pq_norm_t), stream))
+        # live vectors of this shard = set bits of block_valid; the search picks its scan kernel by the mean per cell
+        bits = self.block_valid[:self.n_blocks].view(torch.uint8).long()
+        popc = torch.tensor([bin(i).count("1") for i in range(256)], dtype=torch.long, device=dev)
+        self.set_live(int(popc[bits].sum().item()) if self.n_blocks else 0)
         self.fingerprint = _fingerprint(*self.keep)
         self.stream_id = (stream.value or 0)                                  # searches on another stream wait on `ready`
         self.ready = torch.cuda.Event()
         self.ready.record(torch.cuda.current_stream(dev))
+
+    def set_live(self, n_live: int) -> None:
+        self.n_live = n_live
+        rank, world = self.shard
+        owned = len(range(rank, self.cindex.n_cells, world))
+        self.cindex.mean_cell_live = min(n_live // max(1, owned), 2 ** 31 - 1)
 
     def resident_bytes(self) -> int:
         """Device bytes of the scan layout (what a shard-only rank holds besides the replicated small state)."""
