@@ -70,24 +70,33 @@ def test_add_with_expansion_matches_oracle(cuda_device):
 
 def test_add_updates_scan_layout_in_place(cuda_device):
     """An add that needs no expansion writes the new codes into the existing scan layout (no relayout): the layout object
-    survives, and searches see the new items exactly as a freshly built layout does."""
+    survives, holds the same bytes as a layout built afresh from the reference buffers (the two writers of the format,
+    tpq_store_codes and tpq_relayout_codes, agree on every slot), and searches see the new items exactly as the fresh
+    layout does.  Unsharded, and on shard 1 of 2, where only the shard's cells are written."""
     import torchpq_b200 as T
     torch.manual_seed(8)
     base = torch.randn(64, 30_000, device="cuda")
-    ix = T.IVFPQIndex(64, 16, 32, initial_size=2048, device="cuda:0")
-    ix.train(base[:, :10_000].contiguous())
-    ix.add(base[:, :12_000].contiguous())
-    ix.n_probe = 8
     x = torch.randn(64, 200, device="cuda")
-    ix.search(x, k=10)
-    lay = ix._layout
-    assert lay is not None
-    for s in (12_000, 18_000, 24_000):
-        ix.add(base[:, s:s + 6000].contiguous())
-        assert ix._layout is lay, "the add rebuilt the scan layout"
-    v1, i1, a1 = ix.search(x, k=20, return_address=True)
-    ix._state_changed()                                               # force a relayout from the reference buffers
-    v2, i2, a2 = ix.search(x, k=20, return_address=True)
-    assert ix._layout is not lay
-    assert torch.equal(v1, v2) and torch.equal(i1, i2) and torch.equal(a1, a2)
-    assert int((i1 >= 12_000).sum()) > 0                              # later adds are found
+    for rank, world in ((0, 1), (1, 2)):
+        ix = T.IVFPQIndex(64, 16, 32, initial_size=2048, device="cuda:0")
+        ix.train(base[:, :10_000].contiguous())
+        ix.add(base[:, :12_000].contiguous())
+        ix.set_shard(rank, world)
+        ix.n_probe = 8
+        ix.search(x, k=10)
+        lay = ix._layout
+        assert lay is not None and lay.shard == (rank, world)
+        for s in (12_000, 18_000, 24_000):
+            ix.add(base[:, s:s + 6000].contiguous())
+            assert ix._layout is lay, "the add rebuilt the scan layout"
+        v1, i1, a1 = ix.search(x, k=20, return_address=True)
+        ix._state_changed()                                           # force a relayout from the reference buffers
+        v2, i2, a2 = ix.search(x, k=20, return_address=True)
+        fresh = ix._layout
+        assert fresh is not lay and fresh.shard == (rank, world)
+        assert fresh.n_blocks == lay.n_blocks > 0
+        n_bytes = lay.n_blocks * lay.m_pad * 32
+        assert torch.equal(lay.codes_scan[:n_bytes], fresh.codes_scan[:n_bytes]), (rank, world)
+        assert torch.equal(lay.block_valid[:lay.n_blocks], fresh.block_valid[:fresh.n_blocks]), (rank, world)
+        assert torch.equal(v1, v2) and torch.equal(i1, i2) and torch.equal(a1, a2)
+        assert int((i1 >= 12_000).sum()) > 0                          # later adds are found

@@ -1,6 +1,7 @@
 """CPU model of the cell-major scan (csrc/scan.cu, ivfpq_cell_scan_kernel and its passes): the probe-entry visiting
-rules, the pair list grouped by cell, and bound -> survivors -> select, checked against a plain per-query top-k over
-the entries the query-major kernel visits."""
+rules (probe_count and probe_entry in csrc/scan_layout.cuh, which both scan kernels call), the pair list grouped by
+cell, and bound -> survivors -> select, checked against a plain per-query top-k over the entries the query-major kernel
+visits."""
 import numpy as np
 import pytest
 

@@ -40,7 +40,6 @@ constexpr int AW_N = 128;                         // centroids per N tile
 constexpr int AW_THREADS = 3 * 128;
 constexpr uint32_t AW_STAGE = AW_N * 128;         // one 32-feature slice of an N tile: 128 rows x 128 bytes
 constexpr int AW_MAX_STAGES = 8;
-constexpr int AW_SMEM_LIMIT = 227 * 1024;
 constexpr int AW_K_MAX = 1 << 20;
 
 // D[64 x 128] (+)= A[64 x 8] (registers, TF32) * B[8 x 128] (shared memory, K-major)
@@ -321,7 +320,7 @@ int launch_assign_wide(const float* data, const float* cent, int l, int d, long 
   P.ws = wsf; P.maxsims = maxsims; P.labels = labels;
   const size_t x_bytes = (size_t)AW_M * d * 4;
   const size_t bar_bytes = (2 * AW_MAX_STAGES + 2) * 8;
-  int stages = (int)((AW_SMEM_LIMIT - x_bytes - bar_bytes) / AW_STAGE);
+  int stages = (int)((kSmemLimit - x_bytes - bar_bytes) / AW_STAGE);
   P.stages = stages > AW_MAX_STAGES ? AW_MAX_STAGES : stages;           // >= 6 at d = 256
   const size_t smem = x_bytes + (size_t)P.stages * AW_STAGE + (2 * P.stages + 2) * 8;
   const int sms = device_sm_count();

@@ -255,7 +255,7 @@ extern "C" int tpq_coarse_probe(const float* x_dn, const float* vq_codebook, int
   dim3 grid((n_cells + GB - 1) / GB, (nq + GB - 1) / GB);
   coarse_gemm_kernel<<<grid, 256, 0, st>>>(x_dn, vq_codebook, xn, cn, d, nq, n_cells, sims);
   TPQ_LAUNCH_CHECK("coarse_gemm_kernel");
-  const int kp = next_pow2(n_probe < 32 ? 32 : n_probe);
+  const int kp = list_capacity(n_probe);
   const int wpb = 4;
   size_t smem = (size_t)wpb * (kp + kTopkBuf) * sizeof(uint64_t);
   TPQ_CUDA(cudaFuncSetAttribute(probe_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -22,6 +22,10 @@ int  device_sm_count();
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int next_pow2(int x) { int p = 1; while (p < x) p <<= 1; return p; }
+// slots of a sorted top-k list in shared memory: k rounded up to a power of two, at least one warp's worth
+static inline int list_capacity(int k) { return next_pow2(k < 32 ? 32 : k); }
+// dynamic shared memory one CTA may use on sm_90
+constexpr size_t kSmemLimit = 227 * 1024;
 
 // ----------------------------------------------------------------------------- candidate keys
 // A candidate is one 64-bit key: high word = order-preserving image of the fp32 score,
@@ -50,6 +54,30 @@ __device__ __forceinline__ float    key_score(uint64_t k) { return ord_to_score(
 __device__ __forceinline__ uint32_t key_addr(uint64_t k)  { return 0xFFFFFFFFu - (uint32_t)k; }
 
 #ifdef __CUDACC__
+// One 1024-value tile of a CTA-wide inclusive prefix sum (blockDim.x == 1024, called by every thread): returns carry +
+// the sum of v over threads 0 .. threadIdx.x, and advances carry (shared memory) by the tile's total.  wsum: [32] shared.
+template <class T>
+__device__ __forceinline__ T cta_inclusive_scan(T v, T* wsum, T& carry) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T incl = v;
+  #pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+  if (lane == 31) wsum[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    T w = wsum[lane];
+    #pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += t; }
+    wsum[lane] = w;                                                   // inclusive over warps
+  }
+  __syncthreads();
+  const T r = carry + (warp ? wsum[warp - 1] : T(0)) + incl;
+  __syncthreads();
+  if (threadIdx.x == 1023) carry = r;
+  __syncthreads();
+  return r;
+}
+
 // ----------------------------------------------------------------------------- bitonic networks in registers
 // A warp holds a sequence of 32*R keys as x[r] = element r*32 + lane.  Compare-exchanges at distance >= 32 are
 // register-to-register inside a thread; smaller distances are one SHFL.64 per key -- a quarter of the shared-memory

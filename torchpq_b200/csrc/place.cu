@@ -9,7 +9,7 @@
 // walks the cell slot by slot per ITEM; here: a chunked stable counting sort (one shared-memory bitonic sort per 4096
 // labels + a per-cell scan over chunks), a binary search in a prefix sum of `is_empty` (only when the container has
 // holes), and one scatter kernel that writes the reference layout AND the scan layout (so `add` does not invalidate it).
-#include "common.cuh"
+#include "scan_layout.cuh"
 
 namespace tpq {
 
@@ -106,25 +106,11 @@ scan_u32_inplace_kernel(uint32_t* __restrict__ v, int n) {               // excl
   __shared__ uint32_t carry;
   if (threadIdx.x == 0) carry = 0;
   __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int i0 = 0; i0 < n; i0 += 1024) {
     const int i = i0 + threadIdx.x;
     const uint32_t x = i < n ? v[i] : 0u;
-    uint32_t incl = x;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-    if (lane == 31) wsum[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = wsum[lane];
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += t; }
-      wsum[lane] = w;
-    }
-    __syncthreads();
-    const uint32_t before = carry + (warp ? wsum[warp - 1] : 0u);
-    if (i < n) v[i] = before + incl - x;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry = before + incl;
-    __syncthreads();
+    const uint32_t incl = cta_inclusive_scan(x, wsum, carry);
+    if (i < n) v[i] = incl - x;
   }
 }
 __global__ void __launch_bounds__(EP_T)
@@ -170,7 +156,7 @@ __global__ void write_address_kernel(const int64_t* __restrict__ cells, const in
 // One thread per (item, 4-code word): storage[g][adr] = codes[4g..4g+3][i] (CellContainer.py:213-239); word 0's thread
 // also does the bookkeeping of CellContainer.add's tail (:354-360).  _cell_size is kept as the cell's high-water mark
 // (atomicMax of slot + 1): without holes that IS old size + count.  If a scan layout is given it receives the same codes,
-// lane-rotated (relayout.cu), and the block's valid bit.
+// lane-rotated (scan_layout.cuh), and the block's valid bit.
 __global__ void store_codes_kernel(const uint8_t* __restrict__ codes, const int64_t* __restrict__ cells,
                                    const int64_t* __restrict__ write_adr, const int64_t* __restrict__ ids, int64_t n, int M,
                                    int64_t cap, uint32_t* __restrict__ storage, int64_t* __restrict__ address2id,
@@ -194,15 +180,13 @@ __global__ void store_codes_kernel(const uint8_t* __restrict__ codes, const int6
     is_empty[a] = 0;
     atomicMax(cell_size + c, (long long)(pos + 1));
   }
-  if (codes_scan && (c % shard_world) == shard_rank) {
+  if (codes_scan && shard_owns(c, shard_rank, shard_world)) {
     const int64_t B = (int64_t)cell_block_start[c] + (pos >> 5);
     const int lane = (int)(pos & 31);
-    uint8_t* rec = codes_scan + (size_t)B * MP * 32;
     #pragma unroll
     for (int b = 0; b < 4; ++b) {
-      const int m = 4 * g + b;                                         // record byte t holds sub-quantizer 32*(t/32) + ((lane + t) & 31)
-      const int t = (m & ~31) | ((m - lane) & 31);
-      rec[((size_t)(t >> 4) * 32 + lane) * 16 + (t & 15)] = (uint8_t)(w >> (8 * b));
+      const int t = rot_byte(4 * g + b, lane);
+      codes_scan[scan_chunk_offset(B, MP, t >> 4, lane) + (t & 15)] = (uint8_t)(w >> (8 * b));
     }
     if (g == 0) atomicOr(block_valid + B, 1u << lane);
   }
@@ -300,7 +284,7 @@ extern "C" int tpq_store_codes(const uint8_t* codes, const int64_t* cells, const
               "tpq_store_codes: null pointer");
   const int M = ix->n_subvectors;
   TPQ_REQUIRE(M > 0 && M % 4 == 0, "n_subvectors must be a positive multiple of 4, got %d", M);
-  TPQ_REQUIRE(!codes_scan || (block_valid && ix->cell_block_start && ix->m_pad == (M + 31) / 32 * 32), "tpq_store_codes: incomplete scan layout");
+  TPQ_REQUIRE(!codes_scan || (block_valid && ix->cell_block_start && ix->m_pad == scan_m_pad(M)), "tpq_store_codes: incomplete scan layout");
   dim3 grid((unsigned)((n + 255) / 256), M / 4);
   store_codes_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
       codes, cells, write_adr, ids, n, M, ix->capacity, reinterpret_cast<uint32_t*>(storage), address2id, is_empty,

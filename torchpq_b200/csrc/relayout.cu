@@ -1,19 +1,5 @@
-// Scan ("shadow") layout of the index, derived from the reference's buffers.
-//
-// The reference keeps codes as _storage[M/4, capacity, 4] (container/CellContainer.py:46-53,
-// 213-239): 4-byte granules strided by 4*capacity bytes -- fine for its 4-byte loads
-// (ivfpq_topk.cu:650-660), useless for 128-bit ones.  The scan layout groups every cell's
-// live range [cell_start, cell_start+cell_size) into blocks of 32 vectors; a block is
-// m_pad/16 chunks of 512 bytes, chunk j holding 16 bytes for each of the 32 lanes, so one
-// warp-wide LDG.128 per chunk is a single fully coalesced 512-byte request.
-//
-// Lane l owns vector l of the block.  Its m_pad record bytes are LANE-ROTATED: record byte
-// t (half-group h = t/32, rotation r = t%32) holds the code of sub-quantizer
-//     m(l, t) = 32*h + ((l + r) & 31)
-// so that at any step the 32 lanes of a warp look up 32 different sub-quantizers, i.e. 32
-// different shared-memory banks of the [code][sub-quantizer] LUT (scan.cu) -- every LDS is
-// conflict-free whatever the codes are.  Padding sub-quantizers (m >= M) get code 0.
-#include "common.cuh"
+// Builds the scan layout (format: scan_layout.cuh) and the scan-side codebooks from the reference's buffers.
+#include "scan_layout.cuh"
 
 namespace tpq {
 
@@ -23,30 +9,13 @@ relayout_plan_kernel(const int64_t* __restrict__ cell_size, int C, int rank, int
                      int32_t* __restrict__ cell_block_start) {
   __shared__ int warp_sums[32];
   __shared__ int carry_s;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) { carry_s = 0; cell_block_start[0] = 0; }
+  if (threadIdx.x == 0) { carry_s = 0; cell_block_start[0] = 0; }
   __syncthreads();
   for (int c0 = 0; c0 < C; c0 += 1024) {
-    int c = c0 + tid;
-    int v = 0;
-    if (c < C && (c % world) == rank) { int64_t n = cell_size[c]; v = n > 0 ? (int)((n + 31) >> 5) : 0; }
-    int incl = v;
-    #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int w = warp_sums[lane];
-      #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += t; }
-      warp_sums[lane] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    int base = carry_s + (warp ? warp_sums[warp - 1] : 0);
-    if (c < C) cell_block_start[c + 1] = base + incl;
-    __syncthreads();
-    if (tid == 1023) carry_s = base + incl;
-    __syncthreads();
+    const int c = c0 + threadIdx.x;
+    const int incl = cta_inclusive_scan(c < C && shard_owns(c, rank, world) ? (int)scan_blocks(cell_size[c]) : 0,
+                                        warp_sums, carry_s);
+    if (c < C) cell_block_start[c + 1] = incl;
   }
 }
 
@@ -76,7 +45,6 @@ relayout_codes_kernel(const uint32_t* __restrict__ storage,   // [M/4, cap] word
       *reinterpret_cast<uint32_t*>(rec + lane * row + g * 4) = w;
     }
     __syncwarp();
-    uint8_t* out = codes_scan + (size_t)B * MP * 32;
     for (int j = 0; j < MP / 16; ++j) {
       uint32_t o[4];
       #pragma unroll
@@ -84,14 +52,12 @@ relayout_codes_kernel(const uint32_t* __restrict__ storage,   // [M/4, cap] word
         uint32_t v = 0;
         #pragma unroll
         for (int bb = 0; bb < 4; ++bb) {
-          int t = j * 16 + wd * 4 + bb;
-          int m = (t & ~31) + ((lane + (t & 31)) & 31);
-          uint32_t byte = (m < M) ? rec[lane * row + m] : 0u;
-          v |= byte << (8 * bb);
+          const int m = rot_subq(j * 16 + wd * 4 + bb, lane);
+          v |= ((m < M) ? (uint32_t)rec[lane * row + m] : 0u) << (8 * bb);
         }
         o[wd] = v;
       }
-      *reinterpret_cast<uint4*>(out + ((size_t)j * 32 + lane) * 16) = make_uint4(o[0], o[1], o[2], o[3]);
+      *reinterpret_cast<uint4*>(codes_scan + scan_chunk_offset(B, MP, j, lane)) = make_uint4(o[0], o[1], o[2], o[3]);
     }
     unsigned mask = __ballot_sync(0xffffffffu, live);
     if (lane == 0) block_valid[B] = mask;
@@ -120,8 +86,8 @@ __global__ void __launch_bounds__(256)
 relayout_part2_kernel(const float* __restrict__ vq, const float* __restrict__ pq, int M, int MP, int dsub, int C,
                       float* __restrict__ out) {
   const int c = blockIdx.x, code = threadIdx.x;
-  const int MG = (MP + 63) / 64;
-  float* o = out + (size_t)c * MG * 16384;
+  const int MG = lut_groups(MP);
+  float* o = out + (size_t)c * MG * kLutGroup;
   for (int m = 0; m < MG * 64; ++m) {
     float y = 0.f;
     if (m < M) {
@@ -134,7 +100,7 @@ relayout_part2_kernel(const float* __restrict__ vq, const float* __restrict__ pq
       const float nrm = sqrtf(n2);
       y = __fsub_rn(__fmul_rn(dot, -2.f), __fmul_rn(nrm, nrm));
     }
-    o[(size_t)(m >> 6) * 16384 + code * 64 + (m & 63)] = y;
+    o[lut_index(m, code)] = y;
   }
 }
 
@@ -143,15 +109,14 @@ relayout_part2_kernel(const float* __restrict__ vq, const float* __restrict__ pq
 using namespace tpq;
 
 extern "C" size_t tpq_part2_scan_bytes(int M, int n_cells) {
-  const int MP = (M + 31) / 32 * 32;
-  return (size_t)n_cells * ((MP + 63) / 64) * 65536;
+  return (size_t)n_cells * lut_bytes(scan_m_pad(M));
 }
 
 extern "C" int tpq_relayout_part2(const float* vq_codebook, const float* pq_codebook, int d, int M, int n_cells,
                                   float* part2_scan, void* stream) {
   TPQ_REQUIRE(vq_codebook && pq_codebook && part2_scan, "tpq_relayout_part2: null pointer");
   TPQ_REQUIRE(d > 0 && M > 0 && d % M == 0 && n_cells > 0, "tpq_relayout_part2: bad sizes");
-  const int MP = (M + 31) / 32 * 32;
+  const int MP = scan_m_pad(M);
   relayout_part2_kernel<<<n_cells, 256, 0, (cudaStream_t)stream>>>(vq_codebook, pq_codebook, M, MP, d / M, n_cells, part2_scan);
   TPQ_LAUNCH_CHECK("relayout_part2_kernel");
   return TPQ_OK;
@@ -167,8 +132,7 @@ extern "C" int tpq_relayout_plan(const int64_t* cell_size, int n_cells, int shar
 }
 
 extern "C" size_t tpq_codes_scan_bytes(int M, int64_t n_blocks) {
-  int mp = (M + 31) / 32 * 32;
-  return (size_t)n_blocks * mp * 32;
+  return (size_t)n_blocks * scan_block_bytes(scan_m_pad(M));
 }
 
 extern "C" int tpq_relayout_codes(const tpq_index* ix, uint8_t* codes_scan, uint32_t* block_valid, void* stream) {
@@ -177,7 +141,7 @@ extern "C" int tpq_relayout_codes(const tpq_index* ix, uint8_t* codes_scan, uint
               "tpq_relayout_codes: index is missing reference buffers or the block plan");
   const int M = ix->n_subvectors;
   TPQ_REQUIRE(M > 0 && M % 4 == 0, "n_subvectors must be a positive multiple of 4, got %d", M);
-  const int MP = (M + 31) / 32 * 32;
+  const int MP = scan_m_pad(M);
   TPQ_REQUIRE(ix->m_pad == MP, "index.m_pad=%d, expected %d", ix->m_pad, MP);
   TPQ_REQUIRE(ix->capacity <= 0xFFFFFFFFll, "capacity %lld exceeds the 32-bit address range", (long long)ix->capacity);
   if (ix->n_blocks == 0) return TPQ_OK;
@@ -199,7 +163,7 @@ extern "C" int tpq_relayout_codebook(const float* pq_codebook, int d, int M, int
   TPQ_REQUIRE(pq_codebook && pq_codebook_t && pq_norm_t, "tpq_relayout_codebook: null pointer");
   TPQ_REQUIRE(d > 0 && M > 0 && d % M == 0, "d_vector=%d must be a multiple of n_subvectors=%d", d, M);
   TPQ_REQUIRE(metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE, "tpq_relayout_codebook: unsupported metric %d", metric);
-  const int MP = (M + 31) / 32 * 32;
+  const int MP = scan_m_pad(M);
   int n = 256 * MP;
   relayout_codebook_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(pq_codebook, M, MP, d / M, metric,
                                                                               pq_codebook_t, pq_norm_t);

@@ -5,11 +5,8 @@
 // (IVFPQIndex.py:420-421) and get_id_by_address (container/BaseContainer.py:58-65).
 //
 // Per (query, slice) CTA:
-//   * the query's LUT sits in shared memory TRANSPOSED, lut[g][code][s] (g = m / 64,
-//     s = m % 64, fp32, 256-byte rows), so an entry's byte address is
-//         g*65536 + code*256 + s*4
-//     and, because the codes are lane-rotated (relayout.cu), lane l at step t reads slot
-//     s = 32*(h&1) + ((l + t) & 31): 32 lanes -> 32 distinct banks, zero conflicts.
+//   * the query's LUT sits in shared memory TRANSPOSED, lut[g][code][s] (scan_layout.cuh), and because the codes are
+//     lane-rotated, lane l at step t reads slot s = 32*(h&1) + ((l + t) & 31): 32 lanes -> 32 distinct banks.
 //   * one PRMT builds the whole address: byte 1 = the code byte, byte 0 = the lane's
 //     precomputed slot offset, bytes 2..3 = sign-replicated zero; the half-group and
 //     group offsets are LDS immediates.  Inner loop = PRMT + LDS + FADD per code byte.
@@ -27,7 +24,8 @@
 // -DTPQ_DEBUG_KNOBS build (make dbg -> libtpq_b200_dbg.so, used by scripts/); the product library reads no environment.
 #include <stdlib.h>
 #include <string.h>
-#include "common.cuh"
+#include <type_traits>
+#include "scan_layout.cuh"
 #include "tc_common.cuh"
 
 namespace tpq {
@@ -61,7 +59,7 @@ lut_scan_kernel(const float* __restrict__ x, const float* __restrict__ cb, int d
     a2s[i] = a2;
   }
   __syncthreads();
-  const int MG = (MP + 63) / 64;
+  const int MG = lut_groups(MP);
   for (int mm = 0; mm < LS_MT; ++mm) {
     const int m = m0 + mm;
     if (m >= MP) break;
@@ -79,7 +77,6 @@ lut_scan_kernel(const float* __restrict__ x, const float* __restrict__ cb, int d
         for (int qq = 0; qq < LS_QT; ++qq) dot[qq] = fmaf(xs[(qq * LS_MT + mm) * dsub + e], pv, dot[qq]);
       }
     }
-    const int g = m >> 6, sl = m & 63;
     #pragma unroll
     for (int qq = 0; qq < LS_QT; ++qq) {
       if (q0 + qq >= n_chunk) break;
@@ -89,7 +86,7 @@ lut_scan_kernel(const float* __restrict__ x, const float* __restrict__ cb, int d
         if (metric == TPQ_METRIC_EUCLIDEAN) y = __fsub_rn(__fsub_rn(__fmul_rn(dot[qq], 2.f), a2s[qq * LS_MT + mm]), b2);
         else if (metric == kLutPart1) y = __fmul_rn(dot[qq], 2.f);   // residual IVFPQ: part1 = 2 <x_m, p> (IVFPQIndex.py:377)
       }
-      lut_scan[((size_t)(q0 + qq) * MG + g) * 16384 + c * 64 + sl] = y;
+      lut_scan[(size_t)(q0 + qq) * MG * kLutGroup + lut_index(m, c)] = y;
     }
   }
 }
@@ -118,13 +115,14 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
 // looked up, unit u+1 (the next 64 sub-quantizers of the block, or the first unit of the warp's next block) is in flight.
 template <int MP>
 struct Units {
-  static constexpr int NSB = (MP + 63) / 64;
+  static constexpr int NSB = lut_groups(MP);          // unit u is looked up in LUT group u
   __host__ __device__ static constexpr int words(int sb) { return (sb == NSB - 1 && (MP % 64) != 0) ? 8 : 16; }
 };
 
 template <int MP, int SB>
 __device__ __forceinline__ void load_unit(uint32_t (&w)[16], const uint8_t* __restrict__ codes, int64_t B, int lane) {
-  const uint4* p = reinterpret_cast<const uint4*>(codes + (size_t)B * (MP * 32)) + SB * 128 + lane;
+  // chunks 4 SB .. 4 SB + 3 of block B; lane's 16 bytes of chunk c are uint4 32 c + lane (scan_chunk_offset)
+  const uint4* p = reinterpret_cast<const uint4*>(codes + (size_t)B * scan_block_bytes(MP)) + SB * 128 + lane;
   #pragma unroll
   for (int j = 0; j < Units<MP>::words(SB) / 4; ++j) {
     const uint4 v = ldg_stream(p + j * 32);
@@ -136,7 +134,7 @@ template <int MP, int SB>
 __device__ __forceinline__ void adc_unit(const uint32_t (&w)[16], const uint32_t (&off)[8], const uint8_t* lut, float (&acc)[4]) {
   #pragma unroll
   for (int i = 0; i < Units<MP>::words(SB); ++i) {
-    const int imm = SB * 65536 + (i >> 3) * 128;        // group SB, half-group i/8
+    const int imm = lut_half_group_offset(SB, i >> 3);
     acc[0] += lut_at<0>(lut, w[i], off[i & 7], imm);
     acc[1] += lut_at<1>(lut, w[i], off[i & 7], imm);
     acc[2] += lut_at<2>(lut, w[i], off[i & 7], imm);
@@ -244,8 +242,8 @@ struct Scanner {
 struct ScanSmem { size_t lut, part1, seg_blk0, seg_addr0, seg_cell, seg_prefix, thr, lock, rep, list, bufs, total; };
 static ScanSmem scan_smem(int MP, int n_probe, int nw, int kp, bool residual = false, bool part1_in_smem = false) {
   ScanSmem s; size_t off = 0;
-  s.lut = off;        off += (size_t)((MP + 63) / 64) * 65536;
-  s.part1 = off;      off += (residual && part1_in_smem) ? (size_t)((MP + 63) / 64) * 65536 : 0;   // query half of the residual LUT
+  s.lut = off;        off += lut_bytes(MP);
+  s.part1 = off;      off += (residual && part1_in_smem) ? lut_bytes(MP) : 0;   // query half of the residual LUT
   s.seg_cell = off;   off += residual ? (size_t)n_probe * 4 : 0;
   s.seg_blk0 = off;   off += (size_t)n_probe * 4;
   s.seg_addr0 = off;  off += (size_t)n_probe * 4;
@@ -344,7 +342,7 @@ __device__ __forceinline__ void build_lut(float* lutf, const float* __restrict__
       float y = dot;
       if constexpr (RES) y = __fmul_rn(dot, 2.f);                    // part1 = 2 <x_m, p> (IVFPQIndex.py:377)
       else if (metric == TPQ_METRIC_EUCLIDEAN) y = __fsub_rn(__fsub_rn(__fmul_rn(dot, 2.f), a2[h]), b2);
-      lutf[(h >> 1) * 16384 + c * 64 + (h & 1) * 32 + lane] = y;
+      lutf[lut_index(32 * h + lane, c)] = y;
     }
   }
 }
@@ -363,7 +361,7 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   int32_t*  seg_blk0   = reinterpret_cast<int32_t*>(smem + L.seg_blk0);
   uint32_t* seg_addr0  = reinterpret_cast<uint32_t*>(smem + L.seg_addr0);
   int32_t*  seg_prefix = reinterpret_cast<int32_t*>(smem + L.seg_prefix);
-  constexpr int MG = (MP + 63) / 64;
+  constexpr int MG = lut_groups(MP);
 
   const int qi = blockIdx.x / A.S, slice = blockIdx.x % A.S;  // query within this chunk
   const int q = A.q_base + qi;
@@ -373,10 +371,9 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   long long t_ph = clock64();
 #endif
 
-  // --- probe segments first (warp 0): their dependent global loads overlap the other warps' LUT work (same visiting rules as scan_ref.cu / ivfpq_topk.cu:837-870)
-  int P = (int)A.n_probe_list[q];
-  P = RES ? max(0, min(P, A.n_probe))                         // residual kernel: `for cCell < nProbe` (:1080), may be empty
-          : max(1, min(P, A.n_probe));                        // plain kernel: first cell entered unconditionally
+  // --- probe segments first (warp 0): their dependent global loads overlap the other warps' LUT work (visiting rule:
+  // probe_entry, scan_layout.cuh)
+  const int P = probe_count<RES>(A.n_probe_list[q], A.n_probe);
   int32_t* seg_cell = reinterpret_cast<int32_t*>(smem + L.seg_cell);
   if (warp == 0) {
     int carry = 0;
@@ -386,23 +383,11 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
       const int j = j0 + lane;
       int nb = 0;
       if (j < P) {
-        const int64_t c = cq[j];
-        const bool ok = c >= 0 && c < A.n_cells;            // caller-supplied probe lists (search_cells) are not trusted
-        const int64_t s = ok ? A.cell_start[c] : -1;
-        bool skip = !ok;
-        if (ok && j > 0) {
-          const int64_t cp = cq[j - 1];
-          skip = cp >= 0 && cp < A.n_cells && s == A.cell_start[cp];
-        }
-        const int b0 = ok ? A.cell_block_start[c] : 0;
-        if (!skip) {                                        // the layout holds a block for every slot of the cell's capacity
-          const int have = A.cell_block_start[c + 1] - b0;  // (0 for another shard's cell); the live extent is cell_size
-          const int64_t sz = A.cell_size[c];
-          nb = (int)min((int64_t)have, sz > 0 ? (sz + 31) >> 5 : (int64_t)0);
-        }
-        seg_blk0[j] = b0;
-        seg_addr0[j] = (uint32_t)s;
-        if constexpr (RES) seg_cell[j] = ok ? (int32_t)c : 0;
+        const ProbeEntry e = probe_entry(cq, j, A.n_cells, A.cell_start, A.cell_size, A.cell_block_start);
+        nb = e.nb;
+        seg_blk0[j] = e.blk0;
+        seg_addr0[j] = e.addr0;
+        if constexpr (RES) seg_cell[j] = (int32_t)e.cell;
       }
       int incl = nb;
       #pragma unroll
@@ -415,10 +400,10 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
     // residual with a staged query half: part1 stays in global memory (L2) and is added to part2 cell by cell
   } else if constexpr (DSUB == 0) {
     // --- stage LUT (MG * 64 KB, coalesced 16-byte copies)
-    const float4* src = reinterpret_cast<const float4*>(A.lut_scan + (size_t)qi * MG * 16384);
+    const float4* src = reinterpret_cast<const float4*>(A.lut_scan + (size_t)qi * MG * kLutGroup);
     float4* dst = reinterpret_cast<float4*>(lut);
     #pragma unroll 4
-    for (int i = tid; i < MG * 4096; i += NW * 32) dst[i] = __ldg(src + i);
+    for (int i = tid; i < MG * kLutGroup / 4; i += NW * 32) dst[i] = __ldg(src + i);
   } else {
     // --- build the LUT in place (or, RES, the query half of the residual LUT)
     build_lut<MP, NW, DSUB, RES>(reinterpret_cast<float*>(RES ? smem + L.part1 : lut), A.x, A.cbt, A.M, A.nq, q, A.metric,
@@ -439,14 +424,7 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   sc.tk.init(reinterpret_cast<uint64_t*>(smem + L.list), reinterpret_cast<unsigned long long*>(smem + L.thr),
              reinterpret_cast<int*>(smem + L.lock), reinterpret_cast<uint64_t*>(smem + L.bufs) + (size_t)warp * kStage,
              A.kp, A.k);
-  // lane's slot offsets: byte r%4 of off[r/4] = ((lane + r) & 31) * 4
-  #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    uint32_t v = 0;
-    #pragma unroll
-    for (int b = 0; b < 4; ++b) v |= (uint32_t)(((lane + 4 * i + b) & 31) * 4) << (8 * b);
-    sc.off[i] = v;
-  }
+  lane_slot_offsets(sc.off, lane);
   __syncthreads();
   TPQ_PHASE(0);
 
@@ -460,16 +438,16 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   if constexpr (RES) {
     // query half of the LUT: the shared-memory table built above (DSUB > 0), or the staged copy in global memory
     const float4* p1 = DSUB > 0 ? reinterpret_cast<const float4*>(smem + L.part1)
-                                : reinterpret_cast<const float4*>(A.lut_scan + (size_t)qi * MG * 16384);
+                                : reinterpret_cast<const float4*>(A.lut_scan + (size_t)qi * MG * kLutGroup);
     float4* dst = reinterpret_cast<float4*>(lut);
     for (int j = 0; j < P; ++j) {
       const int b0 = max(seg_prefix[j], b_begin), b1 = min(seg_prefix[j + 1], b_end);
       if (b1 <= b0) continue;                                          // skipped entry, empty cell, another shard's or slice's blocks
       __syncthreads();                                                 // every warp is done with the previous cell's LUT
       if (tid == 0) *sc.next = b0;
-      const float4* p2 = reinterpret_cast<const float4*>(A.part2_scan + (size_t)seg_cell[j] * MG * 16384);
+      const float4* p2 = reinterpret_cast<const float4*>(A.part2_scan + (size_t)seg_cell[j] * MG * kLutGroup);
       #pragma unroll 4
-      for (int i = tid; i < MG * 4096; i += NW * 32) {                 // store_precomputed_to_smem: part1 + part2 (:609-628)
+      for (int i = tid; i < MG * kLutGroup / 4; i += NW * 32) {                 // store_precomputed_to_smem: part1 + part2 (:609-628)
         const float4 a = DSUB > 0 ? p1[i] : __ldg(p1 + i), b = __ldg(p2 + i);
         dst[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
       }
@@ -548,7 +526,7 @@ merge_topk_kernel(const uint64_t* __restrict__ keys_in, int nq, int n_parts, int
 static int launch_merge(const uint64_t* keys_in, int nq, int n_parts, int k, int64_t part_stride, int64_t query_stride,
                         const int64_t* address2id, int64_t capacity, float* values, int64_t* ids, int64_t* address,
                         uint64_t* keys_out, cudaStream_t st) {
-  const int kp = next_pow2(k < 32 ? 32 : k);
+  const int kp = list_capacity(k);
   const int wpb = 4;
   size_t smem = (size_t)wpb * 2 * kp * 8;
   TPQ_CUDA(cudaFuncSetAttribute(merge_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -588,18 +566,6 @@ struct CellArgs {
   int q_base, k, cap;
 };
 
-// the cell of probe entry j >= 1 of query row cq if the query-major kernel scans it (same rules as its prologue), else -1
-__device__ __forceinline__ int64_t visited_cell(const int64_t* cq, int j, int n_cells, const int64_t* cell_start,
-                                                const int64_t* cell_size, const int32_t* cbs) {
-  const int64_t c = cq[j];
-  if (c < 0 || c >= n_cells) return -1;
-  const int64_t cp = cq[j - 1];
-  if (cp >= 0 && cp < n_cells && cell_start[c] == cell_start[cp]) return -1;
-  const int64_t sz = cell_size[c];
-  const int64_t nb = min((int64_t)(cbs[c + 1] - cbs[c]), sz > 0 ? (sz + 31) >> 5 : (int64_t)0);
-  return nb > 0 ? c : -1;
-}
-
 // thread per (query, entry): count the visited pairs of entries 1 .. P-1 per cell; slot = the pair's rank in its cell
 __global__ void cell_pairs_count_kernel(const int64_t* __restrict__ cells, const int64_t* __restrict__ npl, int q_base, int n,
                                         int n_probe, int n_cells, const int64_t* __restrict__ cell_start,
@@ -610,12 +576,10 @@ __global__ void cell_pairs_count_kernel(const int64_t* __restrict__ cells, const
   const int qi = (int)(t / n_probe), j = (int)(t % n_probe);
   const int q = q_base + qi;
   if (j == 0) ones[q] = 1;                                     // pass 1 scans entry 0 only
-  int P = (int)npl[q];
-  P = max(1, min(P, n_probe));
   int pos = -1;
-  if (j >= 1 && j < P) {
-    const int64_t c = visited_cell(cells + (size_t)q * n_probe, j, n_cells, cell_start, cell_size, cbs);
-    if (c >= 0) pos = atomicAdd(cell_cnt + c, 1);
+  if (j >= 1 && j < probe_count<false>(npl[q], n_probe)) {
+    const ProbeEntry e = probe_entry(cells + (size_t)q * n_probe, j, n_cells, cell_start, cell_size, cbs);
+    if (e.nb > 0) pos = atomicAdd(cell_cnt + e.cell, 1);
   }
   slot[t] = pos;
 }
@@ -638,13 +602,12 @@ __global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__
                                                          int* __restrict__ cell_off, CellItem* __restrict__ items,
                                                          int* __restrict__ n_items) {
   __shared__ int hist[kCellBuckets], base[kCellBuckets], warp_sum[32], carry;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   for (int i = tid; i < kCellBuckets; i += 1024) hist[i] = 0;
   if (tid == 0) carry = 0;
   __syncthreads();
   auto chunks_of = [&](int c, int& nb, int& bucket) {
-    const int64_t sz = cell_size[c];
-    nb = (int)min((int64_t)(cbs[c + 1] - cbs[c]), sz > 0 ? (sz + 31) >> 5 : (int64_t)0);
+    nb = cell_blocks(cbs[c], cbs[c + 1], cell_size[c]);
     const int np = cell_cnt[c];
     if (np == 0 || nb == 0) { nb = 0; return 0; }
     const int nch = (nb + kCellChunk - 1) / kCellChunk;
@@ -657,28 +620,15 @@ __global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__
   for (int c0 = 0; c0 < n_cells; c0 += 1024) {
     const int c = c0 + tid;
     const int v = c < n_cells ? cell_cnt[c] : 0;
-    int incl = v;
-    #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += y; }
-    if (lane == 31) warp_sum[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int s = warp_sum[lane], si = s;
-      #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, si, o); if (lane >= o) si += y; }
-      warp_sum[lane] = si - s;
-    }
-    __syncthreads();
+    const int incl = cta_inclusive_scan(v, warp_sum, carry);
     if (c < n_cells) {
-      cell_off[c] = carry + warp_sum[warp] + incl - v;
+      cell_off[c] = incl - v;
       int nb, b;
       const int nch = chunks_of(c, nb, b);
       if (nch) atomicAdd(&hist[b], nch);
     }
-    __syncthreads();
-    if (tid == 1023) carry += warp_sum[31] + incl;
-    __syncthreads();
   }
+  __syncthreads();
   if (tid == 0) {
     int s = 0;
     for (int b = 0; b < kCellBuckets; ++b) { base[b] = s; s += hist[b]; }
@@ -705,33 +655,27 @@ ivfpq_cell_scan_kernel(CellArgs A) {
   constexpr int MP = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* ring = smem;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kCellSlots * 65536);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kCellSlots * lut_bytes(64));
   uint64_t* slot_thr = full + kCellSlots;
   int* slot_q = reinterpret_cast<int*>(slot_thr + kCellSlots);
   int* rel = slot_q + kCellSlots;                              // warps done with the slot's current LUT
   int* item_sh = rel + kCellSlots;                             // [2]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  uint64_t* stage = reinterpret_cast<uint64_t*>(smem + kCellSlots * 65536 + 256) + (size_t)warp * R * 32;
+  uint64_t* stage = reinterpret_cast<uint64_t*>(smem + kCellSlots * lut_bytes(64) + 256) + (size_t)warp * R * 32;
   if (tid == 0) {
     for (int s = 0; s < kCellSlots; ++s) { mbar_init(&full[s], 1); rel[s] = 0; }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   uint32_t off[8];
-  #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    uint32_t v = 0;
-    #pragma unroll
-    for (int b = 0; b < 4; ++b) v |= (uint32_t)(((lane + 4 * i + b) & 31) * 4) << (8 * b);
-    off[i] = v;
-  }
+  lane_slot_offsets(off, lane);
   // one thread: LUT of pair i of the current cell into slot s (every warp has released the slot)
   auto issue = [&](const int32_t* pq, int i, int s) {
     const int qi = pq[i];
     slot_q[s] = qi;
     slot_thr[s] = A.keys[(size_t)(A.q_base + qi) * A.k + A.k - 1];
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the warps' reads of the slot precede the TMA write
-    mbar_expect_tx(&full[s], 65536);
-    bulk_load(ring + s * 65536, A.lut_scan + (size_t)qi * 16384, 65536, &full[s]);
+    mbar_expect_tx(&full[s], lut_bytes(64));
+    bulk_load(ring + s * lut_bytes(64), A.lut_scan + (size_t)qi * kLutGroup, lut_bytes(64), &full[s]);
   };
   uint32_t seq = 0;                                            // LUTs consumed by this CTA so far
   const int n_items = *A.n_items;
@@ -762,7 +706,7 @@ ivfpq_cell_scan_kernel(CellArgs A) {
       mbar_wait(&full[s], (seq / kCellSlots) & 1);
       const int qi = slot_q[s];
       const uint64_t thr = slot_thr[s];
-      const uint8_t* lut = ring + s * 65536;
+      const uint8_t* lut = ring + s * lut_bytes(64);
       int n = 0;
       #pragma unroll
       for (int r = 0; r < R; ++r) {
@@ -804,7 +748,7 @@ ivfpq_cell_scan_kernel(CellArgs A) {
 template <int DSUB>
 __global__ void __launch_bounds__(256) cell_lut_kernel(const float* __restrict__ x, const float* __restrict__ cbt, int M,
                                                        int nq, int q_base, int metric, float* __restrict__ lut) {
-  build_lut<64, 8, DSUB, false>(lut + (size_t)blockIdx.x * 16384, x, cbt, M, nq, q_base + blockIdx.x, metric,
+  build_lut<64, 8, DSUB, false>(lut + (size_t)blockIdx.x * kLutGroup, x, cbt, M, nq, q_base + blockIdx.x, metric,
                                 threadIdx.x & 31, threadIdx.x >> 5);
 }
 
@@ -850,9 +794,8 @@ static bool g_prof_created = false;
 static unsigned long long* g_phase = nullptr;     // device buffer set by tpq_debug_set_phase_buffer (debug build only)
 #endif
 
-static int pick_slices(const tpq_index* ix, int nq, int k) {
+static int pick_slices(int nq) {
   // enough CTAs for ~2 waves of 2 CTAs/SM when the batch is small
-  (void)k;
   const int want = device_sm_count() * 4;
   if (nq >= want) return 1;
   int s = (want + nq - 1) / nq;
@@ -876,8 +819,6 @@ static int fused_dsub(const tpq_index* ix) {
   return (dsub == 1 || dsub == 2 || dsub == 4 || dsub == 8) ? dsub : 0;
 }
 
-struct PeerOut { uint64_t* keys[8]; int n, slot; };
-
 // Cell-major scan when a pair's LUT (64 KB) is clearly smaller than the codes of the cell it meets: the plain index at
 // M <= 64 whose cells hold more than kCellMinLive live vectors (codes) on average, on an unsliced batch.  Unsharded only:
 // on a cell shard, a query's entry 0 is usually another shard's cell, which gives pass 1 no vectors and the bound 0, so
@@ -898,16 +839,15 @@ struct SearchWs {
 // push: the fused-push path (tpq_ivfpq_scan_push), which keeps the query-major kernel
 static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, bool push = false) {
   SearchWs w; size_t off = 0;
-  const int MG = (ix->m_pad + 63) / 64;
   const int chunk = nq < kQueryChunk ? nq : kQueryChunk;
-  const int S = pick_slices(ix, nq, k);
+  const int S = pick_slices(nq);
   const bool cm = !push && cell_major(ix, S);
   w.coarse = off;     off += align_up(tpq_coarse_workspace_bytes(ix->d_vector, nq, ix->n_cells), 256);
   w.probe_sims = off; off += align_up((size_t)nq * n_probe * 4, 256);
   w.cells = off;      off += align_up((size_t)nq * n_probe * 8, 256);
   w.npl = off;        off += align_up((size_t)nq * 8, 256);
   w.xnorm = off;      off += align_up((size_t)nq * ix->d_vector * 4, 256);
-  w.lut = off;        off += fused_dsub(ix) && !cm ? 0 : align_up((size_t)chunk * MG * 65536, 256);
+  w.lut = off;        off += fused_dsub(ix) && !cm ? 0 : align_up((size_t)chunk * lut_bytes(ix->m_pad), 256);
   w.keys = off;       off += align_up((size_t)nq * S * k * 8, 256);
   const size_t C = cm ? (size_t)ix->n_cells : 0, pairs = cm ? (size_t)chunk * n_probe : 0;
   const size_t n_items = cm ? C + (size_t)ix->n_blocks / kCellChunk + 1 : 0;
@@ -923,133 +863,138 @@ static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, bool 
   return w;
 }
 
-static ScanArgs scan_args(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl, int nq, int q0,
-                          int n_probe, int k, int S, const float* lut_ws, uint64_t* keys, const float* base_sims) {
+// One scan of a batch: its queries and probe lists, and where the keys go.  base_sims: the coarse similarities (read by
+// residual IVFPQ); n_peers > 0: the fused exchange into every peer's gather buffer, else the keys go to `keys`.
+struct ScanJob {
+  const tpq_index* ix; const float* x; const int64_t* cells; const int64_t* npl; const float* base_sims;
+  int nq, n_probe, k, S;
+  float* lut_ws; uint64_t* keys; cudaStream_t st; uint64_t* const* peer_keys; int n_peers, peer_slot;
+};
+
+static ScanArgs scan_args(const ScanJob& J, int q0) {
+  const tpq_index* ix = J.ix;
   ScanArgs A;
-  A.x = x; A.cbt = ix->pq_codebook_t; A.M = ix->n_subvectors; A.metric = ix->metric;
-  A.part2_scan = ix->part2_scan; A.base_sims = base_sims;
+  A.x = J.x; A.cbt = ix->pq_codebook_t; A.M = ix->n_subvectors; A.metric = ix->metric; A.part2_scan = ix->part2_scan;
   A.codes = ix->codes_scan; A.valid = ix->block_valid; A.cell_block_start = ix->cell_block_start;
-  A.cell_start = ix->cell_start; A.cell_size = ix->cell_size; A.lut_scan = lut_ws; A.cells = cells; A.n_probe_list = npl; A.keys_out = keys;
-  A.nq = nq; A.q_base = q0; A.n_probe = n_probe; A.k = k; A.kp = next_pow2(k < 32 ? 32 : k); A.S = S;
-  A.boot_r = 2; A.n_cells = ix->n_cells;
-  A.n_peers = 0; A.peer_slot = 0;
+  A.cell_start = ix->cell_start; A.cell_size = ix->cell_size; A.n_cells = ix->n_cells; A.boot_r = 2;
+  A.lut_scan = J.lut_ws; A.cells = J.cells; A.n_probe_list = J.npl; A.base_sims = J.base_sims; A.keys_out = J.keys;
+  A.nq = J.nq; A.q_base = q0; A.n_probe = J.n_probe; A.k = J.k; A.kp = list_capacity(J.k); A.S = J.S;
+  A.n_peers = J.n_peers; A.peer_slot = J.peer_slot;
+  for (int p = 0; p < J.n_peers; ++p) A.peer_keys[p] = J.peer_keys[p];
   A.only_cnt = nullptr; A.only_cap = 0;
   return A;
 }
 
-template <int MP, int NW, int MINB, int DSUB, bool RES = false>
-static int launch_scan_d(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl,
-                         int nq, int n_probe, int k, int S, float* lut_ws, uint64_t* keys, cudaStream_t st,
-                         const float* base_sims = nullptr, const PeerOut* peers = nullptr) {
-  const int kp = next_pow2(k < 32 ? 32 : k);
-  ScanSmem L = scan_smem(MP, n_probe, NW, kp, RES, RES && DSUB > 0);
-  if (L.total > 227 * 1024) {
-    set_error("scan: M=%d n_probe=%d k=%d needs %zu B of shared memory (> 227 KB)", ix->n_subvectors, n_probe, k, L.total);
+// the query-major kernel's shared memory, or an error if a CTA cannot have that much
+static int scan_smem_checked(const ScanJob& J, int MP, int NW, bool residual, bool part1_in_smem, ScanSmem& L) {
+  L = scan_smem(MP, J.n_probe, NW, list_capacity(J.k), residual, part1_in_smem);
+  if (L.total > kSmemLimit) {
+    set_error("scan: M=%d n_probe=%d k=%d needs %zu B of shared memory (> 227 KB)", J.ix->n_subvectors, J.n_probe, J.k, L.total);
     return TPQ_ERR_UNSUPPORTED;
   }
+  return TPQ_OK;
+}
+
+template <int MP, int NW, int MINB, int DSUB, bool RES = false>
+static int launch_scan_d(const ScanJob& J) {
+  const tpq_index* ix = J.ix;
+  ScanSmem L;
+  if (int rc = scan_smem_checked(J, MP, NW, RES, RES && DSUB > 0, L)) return rc;
   auto kern = ivfpq_scan_kernel<MP, NW, MINB, DSUB, RES>;
   TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-  const int MG = (MP + 63) / 64;
-  const int dsub = ix->d_vector / ix->n_subvectors;
-  for (int q0 = 0; q0 < nq; q0 += kQueryChunk) {
-    const int n = (nq - q0) < kQueryChunk ? (nq - q0) : kQueryChunk;
+  for (int q0 = 0; q0 < J.nq; q0 += kQueryChunk) {
+    const int n = (J.nq - q0) < kQueryChunk ? (J.nq - q0) : kQueryChunk;
     if (DSUB == 0) {
-      size_t xs_bytes = (size_t)LS_QT * LS_MT * (dsub + 1) * 4;
+      const size_t xs_bytes = (size_t)LS_QT * LS_MT * (ix->d_vector / ix->n_subvectors + 1) * 4;
       dim3 lgrid((n + LS_QT - 1) / LS_QT, (MP + LS_MT - 1) / LS_MT);
-      lut_scan_kernel<<<lgrid, 256, xs_bytes, st>>>(x, ix->pq_codebook, ix->d_vector, ix->n_subvectors, MP,
-                                                    nq, q0, n, RES ? kLutPart1 : ix->metric, lut_ws);
+      lut_scan_kernel<<<lgrid, 256, xs_bytes, J.st>>>(J.x, ix->pq_codebook, ix->d_vector, ix->n_subvectors, MP,
+                                                      J.nq, q0, n, RES ? kLutPart1 : ix->metric, J.lut_ws);
       TPQ_LAUNCH_CHECK("lut_scan_kernel");
     }
-    ScanArgs A = scan_args(ix, x, cells, npl, nq, q0, n_probe, k, S, lut_ws, keys, base_sims);
-    if (peers) { A.n_peers = peers->n; A.peer_slot = peers->slot; for (int p = 0; p < peers->n; ++p) A.peer_keys[p] = peers->keys[p]; }
+    ScanArgs A = scan_args(J, q0);
 #ifdef TPQ_DEBUG_KNOBS
     { const char* br = getenv("TPQ_BOOT_R"); if (br && atoi(br) == 1) A.boot_r = 1; }
     A.phase = g_phase;
     { const char* bm = getenv("TPQ_BOOT_MODE"); A.boot_mode = bm ? atoi(bm) : 1; }
 #endif
     const bool prof = g_prof_on && g_prof_n < kProfMax;
-    if (prof) cudaEventRecord(g_prof_start[g_prof_n], st);
-    kern<<<n * S, NW * 32, L.total, st>>>(A, L);
-    if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], st);
+    if (prof) cudaEventRecord(g_prof_start[g_prof_n], J.st);
+    kern<<<n * J.S, NW * 32, L.total, J.st>>>(A, L);
+    if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], J.st);
     TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
-    (void)MG; (void)dsub;
   }
   return TPQ_OK;
 }
 
-template <int MP, int NW, int MINB>
-static int launch_scan(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl,
-                       int nq, int n_probe, int k, int S, float* lut_ws, uint64_t* keys, cudaStream_t st, const PeerOut* peers) {
+// f(std::integral_constant<int, DSUB>()) for the index's LUT source (fused_dsub): d/M = 1, 2, 4 or 8, or 0 = staged
+template <class F>
+static int with_dsub(const tpq_index* ix, F&& f) {
   switch (fused_dsub(ix)) {
-    case 1:  return launch_scan_d<MP, NW, MINB, 1>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, nullptr, peers);
-    case 2:  return launch_scan_d<MP, NW, MINB, 2>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, nullptr, peers);
-    case 4:  return launch_scan_d<MP, NW, MINB, 4>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, nullptr, peers);
-    case 8:  return launch_scan_d<MP, NW, MINB, 8>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, nullptr, peers);
-    default: return launch_scan_d<MP, NW, MINB, 0>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, nullptr, peers);
+    case 1:  return f(std::integral_constant<int, 1>());
+    case 2:  return f(std::integral_constant<int, 2>());
+    case 4:  return f(std::integral_constant<int, 4>());
+    case 8:  return f(std::integral_constant<int, 8>());
+    default: return f(std::integral_constant<int, 0>());
   }
 }
 
 // The cell-major scan of a batch (see ivfpq_cell_scan_kernel), per chunk of kQueryChunk queries; leaves keys [nq][k].
 // The profiling events bracket the whole stage: LUTs, pass 1, pair list, pass 2, select and re-run.
 template <int DSUB>
-static int launch_cell_path(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl, int nq,
-                            int n_probe, int k, uint8_t* w, const SearchWs& W, uint64_t* keys, cudaStream_t st) {
-  const int kp = next_pow2(k < 32 ? 32 : k);
-  const int cap = cell_cap(k);
-  const int C = ix->n_cells;
+static int launch_cell_path(const ScanJob& J, uint8_t* w, const SearchWs& W) {
+  const tpq_index* ix = J.ix;
+  const int kp = list_capacity(J.k), cap = cell_cap(J.k), C = ix->n_cells;
+  cudaStream_t st = J.st;
   float* lut_ws = reinterpret_cast<float*>(w + W.lut);
   int* cell_cnt = reinterpret_cast<int*>(w + W.cell_cnt);
   int* n_items = cell_cnt + C;
-  int* cell_off = reinterpret_cast<int*>(w + W.cell_off);
-  int* slot = reinterpret_cast<int*>(w + W.slot);
+  int *cell_off = reinterpret_cast<int*>(w + W.cell_off), *slot = reinterpret_cast<int*>(w + W.slot);
   int* pair_q = reinterpret_cast<int*>(w + W.pair_q);
   CellItem* items = reinterpret_cast<CellItem*>(w + W.items);
   int64_t* ones = reinterpret_cast<int64_t*>(w + W.ones);
   uint64_t* surv = reinterpret_cast<uint64_t*>(w + W.surv);
   int* surv_cnt = reinterpret_cast<int*>(w + W.surv_cnt);
 
-  const ScanSmem L = scan_smem(64, n_probe, 8, kp);
-  if (L.total > 227 * 1024) {
-    set_error("scan: M=%d n_probe=%d k=%d needs %zu B of shared memory (> 227 KB)", ix->n_subvectors, n_probe, k, L.total);
-    return TPQ_ERR_UNSUPPORTED;
-  }
+  ScanSmem L;
+  if (int rc = scan_smem_checked(J, 64, 8, false, false, L)) return rc;
   auto qmajor = ivfpq_scan_kernel<64, 8, 2, 0, false>;                  // 120 registers, 0 spill bytes
   TPQ_CUDA(cudaFuncSetAttribute(qmajor, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
   auto cscan = ivfpq_cell_scan_kernel<kCellNW, kCellR>;
-  const size_t cs_smem = (size_t)kCellSlots * 65536 + 256 + (size_t)kCellChunk * 32 * 8;
+  const size_t cs_smem = (size_t)kCellSlots * lut_bytes(64) + 256 + (size_t)kCellChunk * 32 * 8;
   TPQ_CUDA(cudaFuncSetAttribute(cscan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
   const size_t sel_smem = (size_t)4 * (kp + kTopkBuf) * 8;
   TPQ_CUDA(cudaFuncSetAttribute(cell_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
-  for (int q0 = 0; q0 < nq; q0 += kQueryChunk) {
-    const int n = (nq - q0) < kQueryChunk ? (nq - q0) : kQueryChunk;
+  for (int q0 = 0; q0 < J.nq; q0 += kQueryChunk) {
+    const int n = (J.nq - q0) < kQueryChunk ? (J.nq - q0) : kQueryChunk;
     const bool prof = g_prof_on && g_prof_n < kProfMax;
     if (prof) cudaEventRecord(g_prof_start[g_prof_n], st);
     TPQ_CUDA(cudaMemsetAsync(cell_cnt, 0, (size_t)(C + 2) * 4, st));
     TPQ_CUDA(cudaMemsetAsync(surv_cnt, 0, (size_t)n * 4, st));
-    cell_lut_kernel<DSUB><<<n, 256, 0, st>>>(x, ix->pq_codebook_t, ix->n_subvectors, nq, q0, ix->metric, lut_ws);
+    cell_lut_kernel<DSUB><<<n, 256, 0, st>>>(J.x, ix->pq_codebook_t, ix->n_subvectors, J.nq, q0, ix->metric, lut_ws);
     TPQ_LAUNCH_CHECK("cell_lut_kernel");
-    const int64_t nt = (int64_t)n * n_probe;
+    const int64_t nt = (int64_t)n * J.n_probe;
     const int pgrid = (int)((nt + 255) / 256);
-    cell_pairs_count_kernel<<<pgrid, 256, 0, st>>>(cells, npl, q0, n, n_probe, C, ix->cell_start, ix->cell_size,
+    cell_pairs_count_kernel<<<pgrid, 256, 0, st>>>(J.cells, J.npl, q0, n, J.n_probe, C, ix->cell_start, ix->cell_size,
                                                    ix->cell_block_start, cell_cnt, slot, ones);
     TPQ_LAUNCH_CHECK("cell_pairs_count_kernel");
-    ScanArgs A = scan_args(ix, x, cells, ones, nq, q0, n_probe, k, 1, lut_ws, keys, nullptr);
+    ScanArgs A = scan_args(J, q0);
+    A.n_probe_list = ones;
     qmajor<<<n, 8 * 32, L.total, st>>>(A, L);                              // pass 1: entry 0 of every query
     TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
     cell_plan_kernel<<<1, 1024, 0, st>>>(cell_cnt, ix->cell_block_start, ix->cell_size, C, cell_off, items, n_items);
     TPQ_LAUNCH_CHECK("cell_plan_kernel");
-    cell_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(cells, q0, n, n_probe, slot, cell_off, pair_q);
+    cell_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(J.cells, q0, n, J.n_probe, slot, cell_off, pair_q);
     TPQ_LAUNCH_CHECK("cell_pairs_scatter_kernel");
     CellArgs CA;
     CA.codes = ix->codes_scan; CA.valid = ix->block_valid; CA.cell_block_start = ix->cell_block_start;
     CA.cell_start = ix->cell_start; CA.lut_scan = lut_ws; CA.cell_off = cell_off; CA.cell_cnt = cell_cnt; CA.pair_q = pair_q;
-    CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
-    CA.q_base = q0; CA.k = k; CA.cap = cap;
+    CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = J.keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
+    CA.q_base = q0; CA.k = J.k; CA.cap = cap;
     cscan<<<device_sm_count(), kCellNW * 32, cs_smem, st>>>(CA);
     TPQ_LAUNCH_CHECK("ivfpq_cell_scan_kernel");
-    cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(keys, surv, surv_cnt, q0, n, k, kp, cap);
+    cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(J.keys, surv, surv_cnt, q0, n, J.k, kp, cap);
     TPQ_LAUNCH_CHECK("cell_select_kernel");
-    A.n_probe_list = npl; A.only_cnt = surv_cnt; A.only_cap = cap;
+    A.n_probe_list = J.npl; A.only_cnt = surv_cnt; A.only_cap = cap;
     qmajor<<<n, 8 * 32, L.total, st>>>(A, L);                              // queries whose survivors overflowed
     TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
     if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], st);
@@ -1057,7 +1002,7 @@ static int launch_cell_path(const tpq_index* ix, const float* x, const int64_t* 
   return TPQ_OK;
 }
 
-static int check_index(const tpq_index* ix) {
+static int check_index(const tpq_index* ix, int k) {
   TPQ_REQUIRE(ix, "null index");
   TPQ_REQUIRE(ix->d_vector > 0 && ix->n_subvectors > 0 && ix->d_vector % ix->n_subvectors == 0,
               "d_vector=%d must be a multiple of n_subvectors=%d", ix->d_vector, ix->n_subvectors);
@@ -1068,86 +1013,104 @@ static int check_index(const tpq_index* ix) {
   TPQ_REQUIRE(ix->codes_scan || ix->n_blocks == 0, "index has no scan layout (call tpq_relayout_codes first)");
   TPQ_REQUIRE(ix->block_valid || ix->n_blocks == 0, "index has no scan layout (block_valid)");
   TPQ_REQUIRE(ix->cell_block_start && ix->pq_codebook_t && ix->pq_norm_t, "index has no scan layout (plan / codebook)");
-  TPQ_REQUIRE(ix->m_pad == (ix->n_subvectors + 31) / 32 * 32, "index.m_pad is inconsistent");
+  TPQ_REQUIRE(ix->m_pad == scan_m_pad(ix->n_subvectors), "index.m_pad is inconsistent");
   TPQ_REQUIRE(ix->capacity >= 0 && ix->capacity <= 0xFFFFFFFFll, "capacity exceeds the 32-bit address range");
+  TPQ_REQUIRE(0 < k && k <= 1024, "k must be in (0, 1024], got %d", k);        // IVFPQIndex.py:473
   return TPQ_OK;
 }
 
 // ws/W: the search workspace, for the cell-major path (nullptr: the fused-push path, which keeps the query-major kernel)
-static int scan_dispatch(const tpq_index* ix, const float* x, const int64_t* cells, const int64_t* npl,
-                         int nq, int n_probe, int k, int S, float* lut_ws, uint64_t* keys, cudaStream_t st,
-                         const float* base_sims, uint8_t* ws, const SearchWs* W, const PeerOut* peers = nullptr) {
-  if (ws && !peers && cell_major(ix, S)) {
-#define TPQ_CELL(DS) launch_cell_path<DS>(ix, x, cells, npl, nq, n_probe, k, ws, *W, keys, st)
-    switch (fused_dsub(ix)) {
-      case 1:  return TPQ_CELL(1);
-      case 2:  return TPQ_CELL(2);
-      case 4:  return TPQ_CELL(4);
-      default: return TPQ_CELL(8);
-    }
-#undef TPQ_CELL
-  }
-  if (ix->residual) {
-    // residual IVFPQ.  M <= 64 and d/M in {1,2,4}: the query half of the LUT is built once into a second shared-memory
-    // table (two 64 KB tables -> one 16-warp CTA per SM).  Otherwise (M up to 192, any d/M) the query half is staged in
-    // global memory by lut_scan_kernel and added to the per-cell half straight from L2, so one table suffices.
-    const int dsub = ix->d_vector / ix->n_subvectors;
-    if (!ix->part2_scan || !base_sims) { set_error("residual search needs part2_scan and base_sims"); return TPQ_ERR_BAD_ARG; }
-    if (ix->metric != TPQ_METRIC_EUCLIDEAN) { set_error("residual IVFPQ is defined for the euclidean metric"); return TPQ_ERR_UNSUPPORTED; }
-#define TPQ_RES(MPv, DS) launch_scan_d<MPv, 16, 1, DS, true>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, base_sims, peers)
+static int scan_dispatch(const ScanJob& J, uint8_t* ws, const SearchWs* W) {
+  const tpq_index* ix = J.ix;
+  return with_dsub(ix, [&](auto ds) -> int {
+    constexpr int DS = decltype(ds)::value;
+    if constexpr (DS != 0)                                            // cell_major() implies an in-CTA LUT
+      if (ws && !J.n_peers && cell_major(ix, J.S)) return launch_cell_path<DS>(J, ws, *W);
+    if (ix->residual) {
+      // residual IVFPQ.  M <= 64, d/M in {1,2,4}: the query half of the LUT is built into a second shared-memory table (one
+      // 16-warp CTA per SM).  Otherwise it is staged in global memory and added to the per-cell half from L2.
+      if (!ix->part2_scan || !J.base_sims) { set_error("residual search needs part2_scan and base_sims"); return TPQ_ERR_BAD_ARG; }
+      if (ix->metric != TPQ_METRIC_EUCLIDEAN) { set_error("residual IVFPQ is defined for the euclidean metric"); return TPQ_ERR_UNSUPPORTED; }
 #ifdef TPQ_DEBUG_KNOBS
-    { const char* rm = getenv("TPQ_RES_MODE");                      // A/B: staged query half + 3 light CTAs/SM for M <= 64
-      if (rm && !strcmp(rm, "staged3") && ix->m_pad == 64)
-        return launch_scan_d<64, 8, 3, 0, true>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, base_sims, peers);
-      if (rm && !strcmp(rm, "staged2") && ix->m_pad == 64)
-        return launch_scan_d<64, 8, 2, 0, true>(ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, base_sims, peers); }
+      { const char* rm = getenv("TPQ_RES_MODE");                    // A/B: staged query half + 3 light CTAs/SM for M <= 64
+        if (rm && !strcmp(rm, "staged3") && ix->m_pad == 64) return launch_scan_d<64, 8, 3, 0, true>(J);
+        if (rm && !strcmp(rm, "staged2") && ix->m_pad == 64) return launch_scan_d<64, 8, 2, 0, true>(J); }
 #endif
-    switch (fused_dsub(ix)) {
-      case 1: return ix->m_pad == 32 ? TPQ_RES(32, 1) : TPQ_RES(64, 1);
-      case 2: return ix->m_pad == 32 ? TPQ_RES(32, 2) : TPQ_RES(64, 2);
-      case 4: return ix->m_pad == 32 ? TPQ_RES(32, 4) : TPQ_RES(64, 4);
-      default: break;
+      if constexpr (DS == 1 || DS == 2 || DS == 4)
+        return ix->m_pad == 32 ? launch_scan_d<32, 16, 1, DS, true>(J) : launch_scan_d<64, 16, 1, DS, true>(J);
+      switch (ix->m_pad) {
+        case 32:  return launch_scan_d<32, 16, 1, 0, true>(J);
+        case 64:  return launch_scan_d<64, 16, 1, 0, true>(J);
+        case 96:  return launch_scan_d<96, 16, 1, 0, true>(J);
+        case 128: return launch_scan_d<128, 16, 1, 0, true>(J);
+        case 160: return launch_scan_d<160, 16, 1, 0, true>(J);
+        case 192: return launch_scan_d<192, 16, 1, 0, true>(J);
+        default:
+          set_error("residual IVFPQ: n_subvectors=%d (padded %d) > 192 is not supported", ix->n_subvectors, ix->m_pad);
+          return TPQ_ERR_UNSUPPORTED;
+      }
     }
+#ifdef TPQ_DEBUG_KNOBS
+    // tuning knob for experiments (scripts/sweep_scan.py): TPQ_SCAN_CFG = "<warps>x<min CTAs/SM>"
+    const char* cfg = getenv("TPQ_SCAN_CFG");
+    if (cfg && ix->m_pad == 64) {
+      if (!strcmp(cfg, "8x2"))  return launch_scan_d<64, 8, 2, DS>(J);
+      if (!strcmp(cfg, "8x3"))  return launch_scan_d<64, 8, 3, DS>(J);
+      if (!strcmp(cfg, "16x1")) return launch_scan_d<64, 16, 1, DS>(J);
+      if (!strcmp(cfg, "4x4"))  return launch_scan_d<64, 4, 4, DS>(J);
+    }
+#endif
     switch (ix->m_pad) {
-      case 32:  return TPQ_RES(32, 0);
-      case 64:  return TPQ_RES(64, 0);
-      case 96:  return TPQ_RES(96, 0);
-      case 128: return TPQ_RES(128, 0);
-      case 160: return TPQ_RES(160, 0);
-      case 192: return TPQ_RES(192, 0);
+      case 32:  return launch_scan_d<32, 8, 2, DS>(J);
+      case 64: {
+        // Long probe lists: 2 CTAs/SM with a deep prefetch (127 registers).  Short ones (small cells, or one shard of a
+        // cell-sharded index): per-CTA prologue/epilogue weighs more, so 3 lighter CTAs/SM overlap them better.
+        const double blocks_per_cta = (double)ix->n_blocks / ix->n_cells * J.n_probe / J.S;
+        return blocks_per_cta >= 2000.0 ? launch_scan_d<64, 8, 2, DS>(J) : launch_scan_d<64, 8, 3, DS>(J);
+      }
+      case 96:  return launch_scan_d<96, 16, 1, DS>(J);      // LUT >= 128 KB: one CTA per SM, so twice the warps
+      case 128: return launch_scan_d<128, 16, 1, DS>(J);
+      case 160: return launch_scan_d<160, 16, 1, DS>(J);
+      case 192: return launch_scan_d<192, 16, 1, DS>(J);
       default:
-        set_error("residual IVFPQ: n_subvectors=%d (padded %d) > 192 is not supported", ix->n_subvectors, ix->m_pad);
+        set_error("n_subvectors=%d (padded %d) > 192 is not supported by the scan-layout path", ix->n_subvectors, ix->m_pad);
         return TPQ_ERR_UNSUPPORTED;
     }
-#undef TPQ_RES
+  });
+}
+
+static int check_ws(const SearchWs& W, const void* ws, size_t ws_bytes) {
+  if (!ws || ws_bytes < W.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, W.total); return TPQ_ERR_WORKSPACE; }
+  return TPQ_OK;
+}
+
+// The coarse stage inside the search workspace: cosine queries are normalised (IVFPQIndex.py:474-475), then every query
+// gets its probe list, the lists' similarities and lengths.
+struct Probes { const float* x; const float* sims; const int64_t* cells; const int64_t* npl; };
+static int coarse_stage(const tpq_index* ix, const float* x_dn, int nq, int n_probe, int smart, float temperature,
+                        uint8_t* w, const SearchWs& W, void* stream, Probes& p) {
+  p.x = x_dn;
+  if (ix->metric == TPQ_METRIC_COSINE) {
+    float* xn = reinterpret_cast<float*>(w + W.xnorm);
+    if (int rc = tpq_normalize_columns(x_dn, ix->d_vector, nq, xn, stream)) return rc;
+    p.x = xn;
   }
-#define TPQ_SCAN_ARGS ix, x, cells, npl, nq, n_probe, k, S, lut_ws, keys, st, peers
-#ifdef TPQ_DEBUG_KNOBS
-  // tuning knob for experiments (scripts/sweep_scan.py): TPQ_SCAN_CFG = "<warps>x<min CTAs/SM>"
-  const char* cfg = getenv("TPQ_SCAN_CFG");
-  if (cfg && ix->m_pad == 64) {
-    if (!strcmp(cfg, "8x2"))  return launch_scan<64, 8, 2>(TPQ_SCAN_ARGS);
-    if (!strcmp(cfg, "8x3"))  return launch_scan<64, 8, 3>(TPQ_SCAN_ARGS);
-    if (!strcmp(cfg, "16x1")) return launch_scan<64, 16, 1>(TPQ_SCAN_ARGS);
-    if (!strcmp(cfg, "4x4"))  return launch_scan<64, 4, 4>(TPQ_SCAN_ARGS);
-  }
-#endif
-  switch (ix->m_pad) {
-    case 32:  return launch_scan<32, 8, 2>(TPQ_SCAN_ARGS);
-    case 64: {
-      // Long probe lists: 2 CTAs/SM with a deep prefetch (127 registers).  Short ones (small cells, or one shard of a
-      // cell-sharded index): per-CTA prologue/epilogue weighs more, so 3 lighter CTAs/SM overlap them better.
-      const double blocks_per_cta = (double)ix->n_blocks / ix->n_cells * n_probe / S;
-      return blocks_per_cta >= 2000.0 ? launch_scan<64, 8, 2>(TPQ_SCAN_ARGS) : launch_scan<64, 8, 3>(TPQ_SCAN_ARGS);
-    }
-    case 96:  return launch_scan<96, 16, 1>(TPQ_SCAN_ARGS);      // LUT >= 128 KB: one CTA per SM, so twice the warps
-    case 128: return launch_scan<128, 16, 1>(TPQ_SCAN_ARGS);
-    case 160: return launch_scan<160, 16, 1>(TPQ_SCAN_ARGS);
-    case 192: return launch_scan<192, 16, 1>(TPQ_SCAN_ARGS);
-    default:
-      set_error("n_subvectors=%d (padded %d) > 192 is not supported by the scan-layout path", ix->n_subvectors, ix->m_pad);
-      return TPQ_ERR_UNSUPPORTED;
-  }
+  float* sims = reinterpret_cast<float*>(w + W.probe_sims);
+  int64_t *cells = reinterpret_cast<int64_t*>(w + W.cells), *npl = reinterpret_cast<int64_t*>(w + W.npl);
+  if (int rc = tpq_coarse_probe(p.x, ix->vq_codebook, ix->d_vector, nq, ix->n_cells, n_probe, smart, temperature,
+                                sims, cells, npl, w + W.coarse, W.probe_sims - W.coarse, stream)) return rc;
+  p.sims = sims; p.cells = cells; p.npl = npl;
+  return TPQ_OK;
+}
+
+// scan the batch into the workspace's keys, then merge the slices of every query and decode them
+static int scan_and_merge(const tpq_index* ix, const Probes& p, int nq, int n_probe, int k, uint8_t* w, const SearchWs& W,
+                          float* values, int64_t* ids, int64_t* address, uint64_t* keys_out, cudaStream_t st) {
+  const int S = pick_slices(nq);
+  uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
+  const ScanJob J{ix, p.x, p.cells, p.npl, p.sims, nq, n_probe, k, S, reinterpret_cast<float*>(w + W.lut), keys, st, nullptr, 0, 0};
+  if (int rc = scan_dispatch(J, w, &W)) return rc;
+  return launch_merge(keys, nq, S, k, k, (int64_t)S * k, ix->address2id, ix->capacity, values, ids, address, keys_out, st);
 }
 
 }  // namespace tpq
@@ -1191,88 +1154,55 @@ extern "C" int tpq_ivfpq_search_cells(const tpq_index* ix, const float* x_dn, co
                                       const int64_t* n_probe_list, int nq, int n_probe, int k,
                                       float* values, int64_t* ids, int64_t* address, uint64_t* keys_out,
                                       void* ws, size_t ws_bytes, void* stream) {
-  if (int rc = check_index(ix)) return rc;
-  TPQ_REQUIRE(0 < k && k <= 1024, "k must be in (0, 1024], got %d", k);        // IVFPQIndex.py:473
+  if (int rc = check_index(ix, k)) return rc;
   TPQ_REQUIRE(nq >= 0 && n_probe >= 1, "bad n_query=%d / n_probe=%d", nq, n_probe);
   TPQ_REQUIRE(x_dn && cells && n_probe_list, "null pointer argument");
   if (nq == 0) return TPQ_OK;
-  SearchWs W = search_ws(ix, nq, n_probe, k);
-  if (!ws || ws_bytes < W.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, W.total); return TPQ_ERR_WORKSPACE; }
-  cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  const int S = pick_slices(ix, nq, k);
-  uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
-  if (int rc = scan_dispatch(ix, x_dn, cells, n_probe_list, nq, n_probe, k, S,
-                             reinterpret_cast<float*>(w + W.lut), keys, st, base_sims, w, &W)) return rc;
-  return launch_merge(keys, nq, S, k, k, (int64_t)S * k, ix->address2id, ix->capacity, values, ids, address, keys_out, st);
+  const SearchWs W = search_ws(ix, nq, n_probe, k);
+  if (int rc = check_ws(W, ws, ws_bytes)) return rc;
+  return scan_and_merge(ix, Probes{x_dn, base_sims, cells, n_probe_list}, nq, n_probe, k, reinterpret_cast<uint8_t*>(ws), W,
+                        values, ids, address, keys_out, (cudaStream_t)stream);
 }
 
 extern "C" int tpq_ivfpq_search(const tpq_index* ix, const float* x_dn, int nq, int n_probe, int k,
                                 int smart, float temperature,
                                 float* values, int64_t* ids, int64_t* address, uint64_t* keys_out,
                                 void* ws, size_t ws_bytes, void* stream) {
-  if (int rc = check_index(ix)) return rc;
-  TPQ_REQUIRE(0 < k && k <= 1024, "k must be in (0, 1024], got %d", k);
+  if (int rc = check_index(ix, k)) return rc;
   TPQ_REQUIRE(nq >= 0 && x_dn, "bad query batch");
   TPQ_REQUIRE(n_probe >= 1 && n_probe <= ix->n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, ix->n_cells);
   if (nq == 0) return TPQ_OK;
-  SearchWs W = search_ws(ix, nq, n_probe, k);
-  if (!ws || ws_bytes < W.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, W.total); return TPQ_ERR_WORKSPACE; }
+  const SearchWs W = search_ws(ix, nq, n_probe, k);
+  if (int rc = check_ws(W, ws, ws_bytes)) return rc;
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  const float* x = x_dn;
-  if (ix->metric == TPQ_METRIC_COSINE) {                                        // IVFPQIndex.py:474-475
-    float* xn = reinterpret_cast<float*>(w + W.xnorm);
-    if (int rc = tpq_normalize_columns(x_dn, ix->d_vector, nq, xn, stream)) return rc;
-    x = xn;
-  }
-  float* probe_sims = reinterpret_cast<float*>(w + W.probe_sims);
-  int64_t* cells = reinterpret_cast<int64_t*>(w + W.cells);
-  int64_t* npl = reinterpret_cast<int64_t*>(w + W.npl);
-  if (int rc = tpq_coarse_probe(x, ix->vq_codebook, ix->d_vector, nq, ix->n_cells, n_probe, smart, temperature,
-                                probe_sims, cells, npl, w + W.coarse, W.probe_sims - W.coarse, stream)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int S = pick_slices(ix, nq, k);
-  uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
-  if (int rc = scan_dispatch(ix, x, cells, npl, nq, n_probe, k, S, reinterpret_cast<float*>(w + W.lut), keys, st, probe_sims,
-                             w, &W)) return rc;
-  return launch_merge(keys, nq, S, k, k, (int64_t)S * k, ix->address2id, ix->capacity, values, ids, address, keys_out, st);
+  Probes p;
+  if (int rc = coarse_stage(ix, x_dn, nq, n_probe, smart, temperature, w, W, stream, p)) return rc;
+  return scan_and_merge(ix, p, nq, n_probe, k, w, W, values, ids, address, keys_out, (cudaStream_t)stream);
 }
 
 extern "C" int tpq_ivfpq_scan_push(const tpq_index* ix, const float* x_dn, const int64_t* cells, const float* base_sims,
                                    const int64_t* n_probe_list, int nq, int n_probe, int k, int smart, float temperature,
                                    uint64_t* const* peer_keys, int n_peers, int my_slot,
                                    void* ws, size_t ws_bytes, void* stream) {
-  if (int rc = check_index(ix)) return rc;
-  TPQ_REQUIRE(0 < k && k <= 1024, "k must be in (0, 1024], got %d", k);
+  if (int rc = check_index(ix, k)) return rc;
   TPQ_REQUIRE(nq >= 0 && n_probe >= 1 && x_dn, "bad query batch");
   TPQ_REQUIRE(peer_keys && n_peers >= 1 && n_peers <= 8 && my_slot >= 0, "tpq_ivfpq_scan_push: bad peer list");
   TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "cells and n_probe_list go together");
   if (nq == 0) return TPQ_OK;
-  if (pick_slices(ix, nq, k) != 1) { set_error("tpq_ivfpq_scan_push: batch of %d queries is sliced; use the gathered exchange", nq); return TPQ_ERR_UNSUPPORTED; }
+  if (pick_slices(nq) != 1) { set_error("tpq_ivfpq_scan_push: batch of %d queries is sliced; use the gathered exchange", nq); return TPQ_ERR_UNSUPPORTED; }
   if (nq > kQueryChunk) { set_error("tpq_ivfpq_scan_push: at most %d queries per call", kQueryChunk); return TPQ_ERR_UNSUPPORTED; }
-  SearchWs W = search_ws(ix, nq, n_probe, k, /*push=*/true);
-  if (!ws || ws_bytes < W.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, W.total); return TPQ_ERR_WORKSPACE; }
+  const SearchWs W = search_ws(ix, nq, n_probe, k, /*push=*/true);
+  if (int rc = check_ws(W, ws, ws_bytes)) return rc;
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  const float* x = x_dn;
+  Probes p{x_dn, base_sims, cells, n_probe_list};
   if (!cells) {                                                       // the whole coarse stage runs here (replicated probe)
     TPQ_REQUIRE(n_probe <= ix->n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, ix->n_cells);
-    if (ix->metric == TPQ_METRIC_COSINE) {
-      float* xn = reinterpret_cast<float*>(w + W.xnorm);
-      if (int rc = tpq_normalize_columns(x_dn, ix->d_vector, nq, xn, stream)) return rc;
-      x = xn;
-    }
-    float* probe_sims = reinterpret_cast<float*>(w + W.probe_sims);
-    int64_t* c = reinterpret_cast<int64_t*>(w + W.cells);
-    int64_t* npl = reinterpret_cast<int64_t*>(w + W.npl);
-    if (int rc = tpq_coarse_probe(x, ix->vq_codebook, ix->d_vector, nq, ix->n_cells, n_probe, smart, temperature,
-                                  probe_sims, c, npl, w + W.coarse, W.probe_sims - W.coarse, stream)) return rc;
-    cells = c; n_probe_list = npl; base_sims = probe_sims;
+    if (int rc = coarse_stage(ix, x_dn, nq, n_probe, smart, temperature, w, W, stream, p)) return rc;
   }
-  PeerOut po;
-  po.n = n_peers; po.slot = my_slot;
-  for (int p = 0; p < n_peers; ++p) { TPQ_REQUIRE(peer_keys[p], "null peer buffer"); po.keys[p] = peer_keys[p]; }
-  return scan_dispatch(ix, x, cells, n_probe_list, nq, n_probe, k, 1, reinterpret_cast<float*>(w + W.lut),
-                       reinterpret_cast<uint64_t*>(w + W.keys), (cudaStream_t)stream, base_sims, nullptr, nullptr, &po);
+  for (int i = 0; i < n_peers; ++i) TPQ_REQUIRE(peer_keys[i], "null peer buffer");
+  const ScanJob J{ix, p.x, p.cells, p.npl, p.sims, nq, n_probe, k, 1, reinterpret_cast<float*>(w + W.lut),
+                  reinterpret_cast<uint64_t*>(w + W.keys), (cudaStream_t)stream, peer_keys, n_peers, my_slot};
+  return scan_dispatch(J, nullptr, nullptr);
 }
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k,

@@ -152,11 +152,11 @@ extern "C" int tpq_ivfpq_topk(const uint8_t* data, const float* precomputed, con
   TPQ_REQUIRE((reinterpret_cast<uintptr_t>(data) & 3) == 0 && (reinterpret_cast<uintptr_t>(precomputed) & 15) == 0,
               "data must be 4-byte and precomputed 16-byte aligned");
   if (nq == 0) return TPQ_OK;
-  const int kp = next_pow2(k < 32 ? 32 : k);
+  const int kp = list_capacity(k);
   int nw = 8;
   RefScanSmem L = ref_scan_smem(M, n_probe, nw, kp);
-  while (L.total > 227 * 1024 && nw > 1) { nw >>= 1; L = ref_scan_smem(M, n_probe, nw, kp); }
-  if (L.total > 227 * 1024) {
+  while (L.total > kSmemLimit && nw > 1) { nw >>= 1; L = ref_scan_smem(M, n_probe, nw, kp); }
+  if (L.total > kSmemLimit) {
     set_error("ivfpq_topk: M=%d, n_probe=%d, k=%d needs %zu bytes of shared memory (> 227 KB)", M, n_probe, k, L.total);
     return TPQ_ERR_UNSUPPORTED;
   }
