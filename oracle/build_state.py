@@ -108,6 +108,24 @@ def integer_state(d: int, n_subvectors: int, n_cells: int, n: int, seed: int = 0
     return st, queries
 
 
+def randn_state(d: int, n_subvectors: int, n_cells: int, n: int, seed: int = 0, distance: str = "euclidean",
+                initial_size: int | None = None, scale: float = 1.0) -> O.IndexState:
+    """Real-valued state without training: standard-normal codebooks (times `scale`), random codes and cells, so that
+    LUT entries and scores are arbitrary fp32 values -- for the bit-exact restatements of oracle/fp32_exact.py, where
+    what matters is the arithmetic, not the quality of the quantiser."""
+    rng = np.random.default_rng(seed)
+    M = n_subvectors
+    vq = (rng.standard_normal((d, n_cells)) * scale).astype(np.float32)
+    pq = (rng.standard_normal((M, d // M, 256)) * scale).astype(np.float32)
+    cells = rng.integers(0, n_cells, size=n).astype(np.int64)
+    codes = rng.integers(0, 256, size=(M, n)).astype(np.uint8)
+    if initial_size is None:
+        initial_size = max(1, int(np.bincount(cells, minlength=n_cells).max()))
+    st = O.empty_state(d, M, n_cells, initial_size, distance, vq, pq)
+    O.container_add(st, codes, cells)
+    return st
+
+
 def build_state_residual(base: torch.Tensor, n_subvectors: int, n_cells: int, seed: int = 0, n_train=None,
                          vq_iters: int = 4, pq_iters: int = 3) -> O.IndexState:
     """pq_use_residual=True: PQ is trained on and encodes x - vq_centroid(cell)

@@ -7,10 +7,12 @@
 """
 import numpy as np
 
+from .fp32_exact import fma32
+
 
 def _fma32(a, b, c):
-    """fp32 fused multiply-add emulated through float64 (exact product, one rounding to fp32)."""
-    return (a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64)).astype(np.float32)
+    """fp32 fused multiply-add with one rounding (fp32_exact.fma32: float64 sum, corrected where it double-rounds)."""
+    return fma32(a, b, c)
 
 
 def max_sim(data, cent, distance="euclidean", chunk=4096):

@@ -109,6 +109,8 @@ def test_reference_layout_op(cuda_device):
 
 
 def test_lut_and_coarse(cuda_device):
+    """Against the reference's torch arithmetic, to a tolerance; the bit-exact counterpart, against restatements of
+    these kernels' own arithmetic, is tests/test_fp32_exact_gpu.py."""
     import torchpq_b200 as T
     torch.manual_seed(5)
     for distance in ("euclidean", "cosine"):
