@@ -648,7 +648,9 @@ __global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__
 // Persistent: a CTA takes items (cell, chunk) from a global cursor.  Warp w holds blocks w, w + NW, ... of the chunk
 // (R at most) in registers.  The LUTs of the pairs of the cell arrive by TMA into a ring of kCellSlots 64 KB slots; the
 // last warp to finish with a slot refills it, so no warp waits for another except through the ring.  Per block the
-// scoring is the query-major kernel's adc_unit, so a key is the same bit for bit.
+// scoring is the query-major kernel's adc_unit, so a key is the same bit for bit.  Each lookup is PRMT + LDS + FADD, as
+// in the query-major kernel: the pair body is compiled once per ring slot, so the slot's offset is an LDS immediate
+// and the shared-window base a uniform register (scripts/sass_census.py counts it).
 template <int NW, int R>
 __global__ void __launch_bounds__(NW * 32, 1)
 ivfpq_cell_scan_kernel(CellArgs A) {
@@ -677,7 +679,7 @@ ivfpq_cell_scan_kernel(CellArgs A) {
     mbar_expect_tx(&full[s], lut_bytes(64));
     bulk_load(ring + s * lut_bytes(64), A.lut_scan + (size_t)qi * kLutGroup, lut_bytes(64), &full[s]);
   };
-  uint32_t seq = 0;                                            // LUTs consumed by this CTA so far
+  uint32_t parity = 0;                                         // bit s: phase parity of slot s's next fill
   const int n_items = *A.n_items;
   for (int it = 0;; ++it) {
     if (tid == 0) item_sh[it & 1] = atomicAdd(A.cursor, 1);
@@ -687,11 +689,15 @@ ivfpq_cell_scan_kernel(CellArgs A) {
     const CellItem ci = A.items[item];
     const int np = A.cell_cnt[ci.cell];
     const int32_t* pq = A.pair_q + A.cell_off[ci.cell];
+    // Pair i of every item uses slot i % kCellSlots: the ring is drained at the barrier above, so it can restart at
+    // slot 0, and each pair body below is compiled for its slot (the slot's offset is an LDS immediate).
     if (tid == 0)
-      for (int i = 0; i < min(np, kCellSlots); ++i) issue(pq, i, (seq + i) % kCellSlots);
+      for (int i = 0; i < min(np, kCellSlots); ++i) issue(pq, i, i);
     const int b0 = A.cell_block_start[ci.cell];
     const uint32_t a0 = (uint32_t)A.cell_start[ci.cell];
-    const int nr = (ci.b_hi - ci.b_lo - warp + NW - 1) / NW;   // blocks of this warp (may be <= 0)
+    // blocks of this warp (may be <= 0); broadcast from lane 0 so that the compiler knows it is warp-uniform and the
+    // `r < nr` branches need no divergence handling around the ballots
+    const int nr = __shfl_sync(0xffffffffu, (ci.b_hi - ci.b_lo - warp + NW - 1) / NW, 0);
     uint32_t w[R][16], vmask[R];
     #pragma unroll
     for (int r = 0; r < R; ++r) {
@@ -701,9 +707,10 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         vmask[r] = __ldg(A.valid + B);
       }
     }
-    for (int i = 0; i < np; ++i, ++seq) {
-      const int s = seq % kCellSlots;
-      mbar_wait(&full[s], (seq / kCellSlots) & 1);
+    auto pair = [&](auto slot, int i) {
+      constexpr int s = decltype(slot)::value;
+      mbar_wait(&full[s], (parity >> s) & 1u);
+      parity ^= 1u << s;
       const int qi = slot_q[s];
       const uint64_t thr = slot_thr[s];
       const uint8_t* lut = ring + s * lut_bytes(64);
@@ -740,6 +747,12 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         }
         __syncwarp();
       }
+    };
+    static_assert(kCellSlots == 3, "one pair body per ring slot");
+    for (int i = 0; i < np; i += kCellSlots) {
+      pair(std::integral_constant<int, 0>(), i);
+      if (i + 1 < np) pair(std::integral_constant<int, 1>(), i + 1);
+      if (i + 2 < np) pair(std::integral_constant<int, 2>(), i + 2);
     }
   }
 }
