@@ -807,40 +807,7 @@ static bool g_prof_created = false;
 static unsigned long long* g_phase = nullptr;     // device buffer set by tpq_debug_set_phase_buffer (debug build only)
 #endif
 
-static int pick_slices(int nq) {
-  // enough CTAs for ~2 waves of 2 CTAs/SM when the batch is small
-  const int want = device_sm_count() * 4;
-  if (nq >= want) return 1;
-  int s = (want + nq - 1) / nq;
-  return s > 64 ? 64 : s;
-}
-
-// LUT source: built inside the scan CTA when d/M is 1, 2, 4 or 8 (the codebook slice a CTA reads from L2, M*dsub KB,
-// is then small next to the codes it goes on to stream: C4, d/M = 8, reads 0.98 MB of codebook per 7.5 MB of codes and
-// saves the 2 x 128 KB LUT round trip through HBM plus one launch); staged through HBM by lut_scan_kernel otherwise.
-static int fused_dsub(const tpq_index* ix) {
-  const int dsub = ix->d_vector / ix->n_subvectors;
-#ifdef TPQ_DEBUG_KNOBS
-  const char* mode = getenv("TPQ_LUT_MODE");
-  if (mode && !strcmp(mode, "staged")) return 0;
-#endif
-  // residual IVFPQ keeps TWO tables when the query half is built in the CTA: that fits for M <= 64 and pays for d/M <= 4
-  if (ix->residual && (ix->m_pad > 64 || dsub == 8)) return 0;
-#ifdef TPQ_DEBUG_KNOBS
-  { const char* rm = getenv("TPQ_RES_MODE"); if (ix->residual && rm && !strncmp(rm, "staged", 6)) return 0; }
-#endif
-  return (dsub == 1 || dsub == 2 || dsub == 4 || dsub == 8) ? dsub : 0;
-}
-
-// Cell-major scan when a pair's LUT (64 KB) is clearly smaller than the codes of the cell it meets: the plain index at
-// M <= 64 whose cells hold more than kCellMinLive live vectors (codes) on average, on an unsliced batch.  Unsharded only:
-// on a cell shard, a query's entry 0 is usually another shard's cell, which gives pass 1 no vectors and the bound 0, so
-// every owned candidate would survive and overflow.
-constexpr int kCellMinLive = 1536;
-static bool cell_major(const tpq_index* ix, int S) {
-  return !ix->residual && ix->m_pad == 64 && fused_dsub(ix) && S == 1 && ix->shard_world == 1 && ix->n_blocks > 0 &&
-         ix->mean_cell_live >= kCellMinLive;
-}
+constexpr int kCellMinLive = 1536;    // live vectors per cell, on average, from which the cell-major scan pays
 // survivors kept per query; a query with more is scanned again by the query-major kernel
 static int cell_cap(int k) { return k * 8 > 8192 ? k * 8 : 8192; }
 
@@ -849,20 +816,38 @@ struct SearchWs {
   size_t cell_cnt, cell_off, slot, pair_q, items, ones, surv, surv_cnt;   // cell-major scan only
   size_t total;
 };
-// push: the fused-push path (tpq_ivfpq_scan_push), which keeps the query-major kernel
-static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, bool push = false) {
+
+// What a search of nq queries runs.  plan_scan is the only place that decides it; the workspace size, the launches and
+// the three search entry points all read the plan.
+struct ScanPlan {
+  int S, chunk;                   // CTAs (slices) per query; queries per scan launch
+  bool cell_major;                // the cell-major stage (ivfpq_cell_scan_kernel) instead of one query-major launch
+  int dsub;                       // LUT source: d/M = 1, 2, 4 or 8 when built in the kernel (on the cell-major path:
+                                  // by cell_lut_kernel), 0 = staged through global memory by lut_scan_kernel
+  bool residual, part1_in_smem;   // residual IVFPQ; its query half of the LUT in a second shared-memory table
+  int MP, NW, MINB;               // the query-major kernel: ivfpq_scan_kernel<MP, NW, MINB, qm_dsub(), residual>
+  int boot_r;                     // blocks per warp in the kernel's bootstrap
+#ifdef TPQ_DEBUG_KNOBS
+  int boot_mode; unsigned long long* phase;
+#endif
+  ScanSmem L;                     // the query-major kernel's shared memory
+  SearchWs ws;
+  int rc; char err[160];          // rc != TPQ_OK: the configuration cannot run, and why
+  // the query-major kernel's DSUB: on the cell-major path it reads the LUTs cell_lut_kernel left in the workspace
+  int qm_dsub() const { return cell_major ? 0 : dsub; }
+};
+
+static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, const ScanPlan& P) {
   SearchWs w; size_t off = 0;
-  const int chunk = nq < kQueryChunk ? nq : kQueryChunk;
-  const int S = pick_slices(nq);
-  const bool cm = !push && cell_major(ix, S);
+  const bool cm = P.cell_major;
   w.coarse = off;     off += align_up(tpq_coarse_workspace_bytes(ix->d_vector, nq, ix->n_cells), 256);
   w.probe_sims = off; off += align_up((size_t)nq * n_probe * 4, 256);
   w.cells = off;      off += align_up((size_t)nq * n_probe * 8, 256);
   w.npl = off;        off += align_up((size_t)nq * 8, 256);
   w.xnorm = off;      off += align_up((size_t)nq * ix->d_vector * 4, 256);
-  w.lut = off;        off += fused_dsub(ix) && !cm ? 0 : align_up((size_t)chunk * lut_bytes(ix->m_pad), 256);
-  w.keys = off;       off += align_up((size_t)nq * S * k * 8, 256);
-  const size_t C = cm ? (size_t)ix->n_cells : 0, pairs = cm ? (size_t)chunk * n_probe : 0;
+  w.lut = off;        off += P.qm_dsub() ? 0 : align_up((size_t)P.chunk * lut_bytes(ix->m_pad), 256);
+  w.keys = off;       off += align_up((size_t)nq * P.S * k * 8, 256);
+  const size_t C = cm ? (size_t)ix->n_cells : 0, pairs = cm ? (size_t)P.chunk * n_probe : 0;
   const size_t n_items = cm ? C + (size_t)ix->n_blocks / kCellChunk + 1 : 0;
   w.cell_cnt = off;   off += align_up((C + 2) * 4, 256);                  // pairs per cell, then the item count and cursor
   w.cell_off = off;   off += align_up(C * 4, 256);
@@ -870,95 +855,179 @@ static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, bool 
   w.pair_q = off;     off += align_up(pairs * 4, 256);
   w.items = off;      off += align_up(n_items * sizeof(CellItem), 256);
   w.ones = off;       off += align_up(cm ? (size_t)nq * 8 : 0, 256);
-  w.surv = off;       off += align_up(cm ? (size_t)chunk * cell_cap(k) * 8 : 0, 256);
-  w.surv_cnt = off;   off += align_up(cm ? (size_t)chunk * 4 : 0, 256);
+  w.surv = off;       off += align_up(cm ? (size_t)P.chunk * cell_cap(k) * 8 : 0, 256);
+  w.surv_cnt = off;   off += align_up(cm ? (size_t)P.chunk * 4 : 0, 256);
   w.total = off;
   return w;
 }
 
-// One scan of a batch: its queries and probe lists, and where the keys go.  base_sims: the coarse similarities (read by
-// residual IVFPQ); n_peers > 0: the fused exchange into every peer's gather buffer, else the keys go to `keys`.
+// push: the fused-push path (tpq_ivfpq_scan_push), which keeps the query-major kernel
+static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool push) {
+  ScanPlan P{};
+  const int dsub = ix->d_vector / ix->n_subvectors;
+  const int want = device_sm_count() * 4;       // enough CTAs for ~2 waves of 2 CTAs/SM when the batch is small
+  P.S = nq >= want ? 1 : ((want + nq - 1) / nq > 64 ? 64 : (want + nq - 1) / nq);
+  P.chunk = nq < kQueryChunk ? nq : kQueryChunk;
+  P.residual = ix->residual != 0;
+  P.MP = ix->m_pad;
+  P.boot_r = 2;
+  // LUT source: built inside the scan CTA when d/M is 1, 2, 4 or 8 (the codebook slice a CTA reads from L2, M*dsub KB,
+  // is then small next to the codes it goes on to stream: C4, d/M = 8, reads 0.98 MB of codebook per 7.5 MB of codes
+  // and saves the 2 x 128 KB LUT round trip through HBM plus one launch); staged through HBM by lut_scan_kernel
+  // otherwise.  Residual IVFPQ keeps TWO tables when the query half is built in the CTA: that fits for M <= 64 and pays
+  // for d/M <= 4.
+  P.dsub = (dsub == 1 || dsub == 2 || dsub == 4 || dsub == 8) ? dsub : 0;
+  if (P.residual && (P.MP > 64 || dsub == 8)) P.dsub = 0;
+  if (P.residual || P.MP > 64) {
+    // residual: one 16-warp CTA per SM; M > 64: the LUT is >= 128 KB, so one CTA per SM with twice the warps
+    P.NW = 16; P.MINB = 1;
+  } else if (P.MP == 64) {
+    // Long probe lists: 2 CTAs/SM with a deep prefetch (127 registers).  Short ones (small cells, or one shard of a
+    // cell-sharded index): per-CTA prologue/epilogue weighs more, so 3 lighter CTAs/SM overlap them better.
+    const double blocks_per_cta = (double)ix->n_blocks / ix->n_cells * n_probe / P.S;
+    P.NW = 8; P.MINB = blocks_per_cta >= 2000.0 ? 2 : 3;
+  } else {
+    P.NW = 8; P.MINB = 2;
+  }
+#ifdef TPQ_DEBUG_KNOBS
+  // experiment knobs (scripts/sweep_scan.py), read once per search
+  const char* lm = getenv("TPQ_LUT_MODE");            // "staged": every LUT through lut_scan_kernel
+  if (lm && !strcmp(lm, "staged")) P.dsub = 0;
+  const char* rm = getenv("TPQ_RES_MODE");            // residual, "staged*": the query half through lut_scan_kernel,
+  if (P.residual && rm && !strncmp(rm, "staged", 6)) {  // "staged2|3": with 8-warp CTAs, 2|3 per SM, at M <= 64
+    P.dsub = 0;
+    if (P.MP == 64 && !strcmp(rm, "staged3")) { P.NW = 8; P.MINB = 3; }
+    if (P.MP == 64 && !strcmp(rm, "staged2")) { P.NW = 8; P.MINB = 2; }
+  }
+  const char* cfg = getenv("TPQ_SCAN_CFG");           // "<warps>x<min CTAs/SM>" of the plain query-major kernel at M <= 64
+  if (cfg && !P.residual && P.MP == 64) {
+    if (!strcmp(cfg, "8x2"))  { P.NW = 8;  P.MINB = 2; }
+    if (!strcmp(cfg, "8x3"))  { P.NW = 8;  P.MINB = 3; }
+    if (!strcmp(cfg, "16x1")) { P.NW = 16; P.MINB = 1; }
+    if (!strcmp(cfg, "4x4"))  { P.NW = 4;  P.MINB = 4; }
+  }
+  const char* br = getenv("TPQ_BOOT_R");
+  if (br && atoi(br) == 1) P.boot_r = 1;
+  const char* bm = getenv("TPQ_BOOT_MODE");
+  P.boot_mode = bm ? atoi(bm) : 1;
+  P.phase = g_phase;
+#endif
+  // Cell-major scan when a pair's LUT (64 KB) is clearly smaller than the codes of the cell it meets: the plain index at
+  // M <= 64, with an in-kernel LUT build, whose cells hold more than kCellMinLive live vectors (codes) on average, on an
+  // unsliced batch.  Unsharded only: on a cell shard, a query's entry 0 is usually another shard's cell, which gives
+  // pass 1 no vectors and the bound 0, so every owned candidate would survive and overflow.
+  P.cell_major = !push && !P.residual && P.MP == 64 && P.dsub && P.S == 1 && ix->shard_world == 1 && ix->n_blocks > 0 &&
+                 ix->mean_cell_live >= kCellMinLive;
+  if (P.cell_major) { P.NW = 8; P.MINB = 2; }        // pass 1 and the overflow re-run: 120 registers, 0 spill bytes
+  P.part1_in_smem = P.residual && P.dsub > 0;
+  P.L = scan_smem(P.MP, n_probe, P.NW, list_capacity(k), P.residual, P.part1_in_smem);
+  P.ws = search_ws(ix, nq, n_probe, k, P);
+  if (P.residual && ix->metric != TPQ_METRIC_EUCLIDEAN) {
+    P.rc = TPQ_ERR_UNSUPPORTED;
+    snprintf(P.err, sizeof P.err, "residual IVFPQ is defined for the euclidean metric");
+  } else if (P.MP > 192) {
+    P.rc = TPQ_ERR_UNSUPPORTED;
+    if (P.residual)
+      snprintf(P.err, sizeof P.err, "residual IVFPQ: n_subvectors=%d (padded %d) > 192 is not supported", ix->n_subvectors, P.MP);
+    else
+      snprintf(P.err, sizeof P.err, "n_subvectors=%d (padded %d) > 192 is not supported by the scan-layout path", ix->n_subvectors, P.MP);
+  } else if (P.L.total > kSmemLimit) {
+    P.rc = TPQ_ERR_UNSUPPORTED;
+    snprintf(P.err, sizeof P.err, "scan: M=%d n_probe=%d k=%d needs %zu B of shared memory (> 227 KB)", ix->n_subvectors, n_probe, k, P.L.total);
+  }
+  return P;
+}
+
+// The plan's query-major kernel.  The instantiations named here are all that exist; plan_scan picks among them.
+using ScanKernel = void (*)(ScanArgs, ScanSmem);
+template <int DSUB>
+static ScanKernel scan_kernel_d(const ScanPlan& P) {
+  if (P.residual) {
+    if constexpr (DSUB == 1 || DSUB == 2 || DSUB == 4)
+      return P.MP == 32 ? ivfpq_scan_kernel<32, 16, 1, DSUB, true> : ivfpq_scan_kernel<64, 16, 1, DSUB, true>;
+#ifdef TPQ_DEBUG_KNOBS
+    if (P.MP == 64 && P.NW == 8) return P.MINB == 3 ? ivfpq_scan_kernel<64, 8, 3, 0, true> : ivfpq_scan_kernel<64, 8, 2, 0, true>;
+#endif
+    switch (P.MP) {
+      case 32:  return ivfpq_scan_kernel<32, 16, 1, 0, true>;
+      case 64:  return ivfpq_scan_kernel<64, 16, 1, 0, true>;
+      case 96:  return ivfpq_scan_kernel<96, 16, 1, 0, true>;
+      case 128: return ivfpq_scan_kernel<128, 16, 1, 0, true>;
+      case 160: return ivfpq_scan_kernel<160, 16, 1, 0, true>;
+      case 192: return ivfpq_scan_kernel<192, 16, 1, 0, true>;
+    }
+    return nullptr;
+  }
+#ifdef TPQ_DEBUG_KNOBS
+  if (P.MP == 64 && P.NW == 16) return ivfpq_scan_kernel<64, 16, 1, DSUB, false>;
+  if (P.MP == 64 && P.NW == 4)  return ivfpq_scan_kernel<64, 4, 4, DSUB, false>;
+#endif
+  switch (P.MP) {
+    case 32:  return ivfpq_scan_kernel<32, 8, 2, DSUB, false>;
+    case 64:  return P.MINB == 2 ? ivfpq_scan_kernel<64, 8, 2, DSUB, false> : ivfpq_scan_kernel<64, 8, 3, DSUB, false>;
+    case 96:  return ivfpq_scan_kernel<96, 16, 1, DSUB, false>;
+    case 128: return ivfpq_scan_kernel<128, 16, 1, DSUB, false>;
+    case 160: return ivfpq_scan_kernel<160, 16, 1, DSUB, false>;
+    case 192: return ivfpq_scan_kernel<192, 16, 1, DSUB, false>;
+  }
+  return nullptr;
+}
+static ScanKernel scan_kernel(const ScanPlan& P) {
+  switch (P.qm_dsub()) {
+    case 1:  return scan_kernel_d<1>(P);
+    case 2:  return scan_kernel_d<2>(P);
+    case 4:  return scan_kernel_d<4>(P);
+    case 8:  return scan_kernel_d<8>(P);
+    default: return scan_kernel_d<0>(P);
+  }
+}
+using CellLutKernel = decltype(&cell_lut_kernel<1>);
+static CellLutKernel cell_lut(int dsub) {                    // the cell-major path builds its LUTs in-kernel only
+  switch (dsub) {
+    case 1:  return cell_lut_kernel<1>;
+    case 2:  return cell_lut_kernel<2>;
+    case 4:  return cell_lut_kernel<4>;
+    default: return cell_lut_kernel<8>;
+  }
+}
+
+// One scan of a batch: its queries and probe lists, and the search workspace w.  base_sims: the coarse similarities
+// (read by residual IVFPQ); n_peers > 0: the fused exchange into every peer's gather buffer, else the keys go to the
+// workspace's keys [nq][S][k].
 struct ScanJob {
   const tpq_index* ix; const float* x; const int64_t* cells; const int64_t* npl; const float* base_sims;
-  int nq, n_probe, k, S;
-  float* lut_ws; uint64_t* keys; cudaStream_t st; uint64_t* const* peer_keys; int n_peers, peer_slot;
+  int nq, n_probe, k;
+  uint8_t* w; cudaStream_t st; uint64_t* const* peer_keys; int n_peers, peer_slot;
 };
 
-static ScanArgs scan_args(const ScanJob& J, int q0) {
+// the arguments of every query-major launch for the chunk at q0
+static ScanArgs scan_args(const ScanPlan& P, const ScanJob& J, int q0) {
   const tpq_index* ix = J.ix;
-  ScanArgs A;
+  ScanArgs A{};
   A.x = J.x; A.cbt = ix->pq_codebook_t; A.M = ix->n_subvectors; A.metric = ix->metric; A.part2_scan = ix->part2_scan;
   A.codes = ix->codes_scan; A.valid = ix->block_valid; A.cell_block_start = ix->cell_block_start;
-  A.cell_start = ix->cell_start; A.cell_size = ix->cell_size; A.n_cells = ix->n_cells; A.boot_r = 2;
-  A.lut_scan = J.lut_ws; A.cells = J.cells; A.n_probe_list = J.npl; A.base_sims = J.base_sims; A.keys_out = J.keys;
-  A.nq = J.nq; A.q_base = q0; A.n_probe = J.n_probe; A.k = J.k; A.kp = list_capacity(J.k); A.S = J.S;
+  A.cell_start = ix->cell_start; A.cell_size = ix->cell_size; A.n_cells = ix->n_cells; A.boot_r = P.boot_r;
+  A.lut_scan = reinterpret_cast<const float*>(J.w + P.ws.lut); A.cells = J.cells; A.n_probe_list = J.npl;
+  A.base_sims = J.base_sims; A.keys_out = reinterpret_cast<uint64_t*>(J.w + P.ws.keys);
+  A.nq = J.nq; A.q_base = q0; A.n_probe = J.n_probe; A.k = J.k; A.kp = list_capacity(J.k); A.S = P.S;
   A.n_peers = J.n_peers; A.peer_slot = J.peer_slot;
   for (int p = 0; p < J.n_peers; ++p) A.peer_keys[p] = J.peer_keys[p];
-  A.only_cnt = nullptr; A.only_cap = 0;
+#ifdef TPQ_DEBUG_KNOBS
+  A.phase = P.phase; A.boot_mode = P.boot_mode;
+#endif
   return A;
 }
 
-// the query-major kernel's shared memory, or an error if a CTA cannot have that much
-static int scan_smem_checked(const ScanJob& J, int MP, int NW, bool residual, bool part1_in_smem, ScanSmem& L) {
-  L = scan_smem(MP, J.n_probe, NW, list_capacity(J.k), residual, part1_in_smem);
-  if (L.total > kSmemLimit) {
-    set_error("scan: M=%d n_probe=%d k=%d needs %zu B of shared memory (> 227 KB)", J.ix->n_subvectors, J.n_probe, J.k, L.total);
-    return TPQ_ERR_UNSUPPORTED;
-  }
-  return TPQ_OK;
-}
-
-template <int MP, int NW, int MINB, int DSUB, bool RES = false>
-static int launch_scan_d(const ScanJob& J) {
+// The cell-major scan of the n queries at q0 (see ivfpq_cell_scan_kernel); leaves their keys [n][k].  qmajor and A:
+// the plan's query-major kernel and its arguments for the chunk, for pass 1 and the overflow re-run.
+static int cell_stage(const ScanPlan& P, const ScanJob& J, ScanKernel qmajor, ScanArgs A, int q0, int n) {
   const tpq_index* ix = J.ix;
-  ScanSmem L;
-  if (int rc = scan_smem_checked(J, MP, NW, RES, RES && DSUB > 0, L)) return rc;
-  auto kern = ivfpq_scan_kernel<MP, NW, MINB, DSUB, RES>;
-  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-  for (int q0 = 0; q0 < J.nq; q0 += kQueryChunk) {
-    const int n = (J.nq - q0) < kQueryChunk ? (J.nq - q0) : kQueryChunk;
-    if (DSUB == 0) {
-      const size_t xs_bytes = (size_t)LS_QT * LS_MT * (ix->d_vector / ix->n_subvectors + 1) * 4;
-      dim3 lgrid((n + LS_QT - 1) / LS_QT, (MP + LS_MT - 1) / LS_MT);
-      lut_scan_kernel<<<lgrid, 256, xs_bytes, J.st>>>(J.x, ix->pq_codebook, ix->d_vector, ix->n_subvectors, MP,
-                                                      J.nq, q0, n, RES ? kLutPart1 : ix->metric, J.lut_ws);
-      TPQ_LAUNCH_CHECK("lut_scan_kernel");
-    }
-    ScanArgs A = scan_args(J, q0);
-#ifdef TPQ_DEBUG_KNOBS
-    { const char* br = getenv("TPQ_BOOT_R"); if (br && atoi(br) == 1) A.boot_r = 1; }
-    A.phase = g_phase;
-    { const char* bm = getenv("TPQ_BOOT_MODE"); A.boot_mode = bm ? atoi(bm) : 1; }
-#endif
-    const bool prof = g_prof_on && g_prof_n < kProfMax;
-    if (prof) cudaEventRecord(g_prof_start[g_prof_n], J.st);
-    kern<<<n * J.S, NW * 32, L.total, J.st>>>(A, L);
-    if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], J.st);
-    TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
-  }
-  return TPQ_OK;
-}
-
-// f(std::integral_constant<int, DSUB>()) for the index's LUT source (fused_dsub): d/M = 1, 2, 4 or 8, or 0 = staged
-template <class F>
-static int with_dsub(const tpq_index* ix, F&& f) {
-  switch (fused_dsub(ix)) {
-    case 1:  return f(std::integral_constant<int, 1>());
-    case 2:  return f(std::integral_constant<int, 2>());
-    case 4:  return f(std::integral_constant<int, 4>());
-    case 8:  return f(std::integral_constant<int, 8>());
-    default: return f(std::integral_constant<int, 0>());
-  }
-}
-
-// The cell-major scan of a batch (see ivfpq_cell_scan_kernel), per chunk of kQueryChunk queries; leaves keys [nq][k].
-// The profiling events bracket the whole stage: LUTs, pass 1, pair list, pass 2, select and re-run.
-template <int DSUB>
-static int launch_cell_path(const ScanJob& J, uint8_t* w, const SearchWs& W) {
-  const tpq_index* ix = J.ix;
+  const SearchWs& W = P.ws;
+  uint8_t* w = J.w;
   const int kp = list_capacity(J.k), cap = cell_cap(J.k), C = ix->n_cells;
   cudaStream_t st = J.st;
   float* lut_ws = reinterpret_cast<float*>(w + W.lut);
+  uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
   int* cell_cnt = reinterpret_cast<int*>(w + W.cell_cnt);
   int* n_items = cell_cnt + C;
   int *cell_off = reinterpret_cast<int*>(w + W.cell_off), *slot = reinterpret_cast<int*>(w + W.slot);
@@ -968,49 +1037,69 @@ static int launch_cell_path(const ScanJob& J, uint8_t* w, const SearchWs& W) {
   uint64_t* surv = reinterpret_cast<uint64_t*>(w + W.surv);
   int* surv_cnt = reinterpret_cast<int*>(w + W.surv_cnt);
 
-  ScanSmem L;
-  if (int rc = scan_smem_checked(J, 64, 8, false, false, L)) return rc;
-  auto qmajor = ivfpq_scan_kernel<64, 8, 2, 0, false>;                  // 120 registers, 0 spill bytes
-  TPQ_CUDA(cudaFuncSetAttribute(qmajor, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
   auto cscan = ivfpq_cell_scan_kernel<kCellNW, kCellR>;
   const size_t cs_smem = (size_t)kCellSlots * lut_bytes(64) + 256 + (size_t)kCellChunk * 32 * 8;
   TPQ_CUDA(cudaFuncSetAttribute(cscan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
   const size_t sel_smem = (size_t)4 * (kp + kTopkBuf) * 8;
   TPQ_CUDA(cudaFuncSetAttribute(cell_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
-  for (int q0 = 0; q0 < J.nq; q0 += kQueryChunk) {
-    const int n = (J.nq - q0) < kQueryChunk ? (J.nq - q0) : kQueryChunk;
+  TPQ_CUDA(cudaMemsetAsync(cell_cnt, 0, (size_t)(C + 2) * 4, st));
+  TPQ_CUDA(cudaMemsetAsync(surv_cnt, 0, (size_t)n * 4, st));
+  cell_lut(P.dsub)<<<n, 256, 0, st>>>(J.x, ix->pq_codebook_t, ix->n_subvectors, J.nq, q0, ix->metric, lut_ws);
+  TPQ_LAUNCH_CHECK("cell_lut_kernel");
+  const int64_t nt = (int64_t)n * J.n_probe;
+  const int pgrid = (int)((nt + 255) / 256);
+  cell_pairs_count_kernel<<<pgrid, 256, 0, st>>>(J.cells, J.npl, q0, n, J.n_probe, C, ix->cell_start, ix->cell_size,
+                                                 ix->cell_block_start, cell_cnt, slot, ones);
+  TPQ_LAUNCH_CHECK("cell_pairs_count_kernel");
+  A.n_probe_list = ones;
+  qmajor<<<n, P.NW * 32, P.L.total, st>>>(A, P.L);                        // pass 1: entry 0 of every query
+  TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
+  cell_plan_kernel<<<1, 1024, 0, st>>>(cell_cnt, ix->cell_block_start, ix->cell_size, C, cell_off, items, n_items);
+  TPQ_LAUNCH_CHECK("cell_plan_kernel");
+  cell_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(J.cells, q0, n, J.n_probe, slot, cell_off, pair_q);
+  TPQ_LAUNCH_CHECK("cell_pairs_scatter_kernel");
+  CellArgs CA;
+  CA.codes = ix->codes_scan; CA.valid = ix->block_valid; CA.cell_block_start = ix->cell_block_start;
+  CA.cell_start = ix->cell_start; CA.lut_scan = lut_ws; CA.cell_off = cell_off; CA.cell_cnt = cell_cnt; CA.pair_q = pair_q;
+  CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
+  CA.q_base = q0; CA.k = J.k; CA.cap = cap;
+  cscan<<<device_sm_count(), kCellNW * 32, cs_smem, st>>>(CA);
+  TPQ_LAUNCH_CHECK("ivfpq_cell_scan_kernel");
+  cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(keys, surv, surv_cnt, q0, n, J.k, kp, cap);
+  TPQ_LAUNCH_CHECK("cell_select_kernel");
+  A.n_probe_list = J.npl; A.only_cnt = surv_cnt; A.only_cap = cap;
+  qmajor<<<n, P.NW * 32, P.L.total, st>>>(A, P.L);                        // queries whose survivors overflowed
+  TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
+  return TPQ_OK;
+}
+
+// Every scan launch of a batch, per chunk of P.chunk queries: the cell-major stage, or the staged LUT (when there is
+// one) and the query-major kernel.  The profiling events bracket the scan stage of each chunk: the whole cell-major
+// stage, or the query-major kernel.
+static int launch(const ScanPlan& P, const ScanJob& J) {
+  const tpq_index* ix = J.ix;
+  const ScanKernel kern = scan_kernel(P);
+  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.L.total));
+  for (int q0 = 0; q0 < J.nq; q0 += P.chunk) {
+    const int n = (J.nq - q0) < P.chunk ? (J.nq - q0) : P.chunk;
+    if (!P.cell_major && P.dsub == 0) {
+      const size_t xs_bytes = (size_t)LS_QT * LS_MT * (ix->d_vector / ix->n_subvectors + 1) * 4;
+      dim3 lgrid((n + LS_QT - 1) / LS_QT, (P.MP + LS_MT - 1) / LS_MT);
+      lut_scan_kernel<<<lgrid, 256, xs_bytes, J.st>>>(J.x, ix->pq_codebook, ix->d_vector, ix->n_subvectors, P.MP, J.nq,
+                                                      q0, n, P.residual ? kLutPart1 : ix->metric,
+                                                      reinterpret_cast<float*>(J.w + P.ws.lut));
+      TPQ_LAUNCH_CHECK("lut_scan_kernel");
+    }
+    const ScanArgs A = scan_args(P, J, q0);
     const bool prof = g_prof_on && g_prof_n < kProfMax;
-    if (prof) cudaEventRecord(g_prof_start[g_prof_n], st);
-    TPQ_CUDA(cudaMemsetAsync(cell_cnt, 0, (size_t)(C + 2) * 4, st));
-    TPQ_CUDA(cudaMemsetAsync(surv_cnt, 0, (size_t)n * 4, st));
-    cell_lut_kernel<DSUB><<<n, 256, 0, st>>>(J.x, ix->pq_codebook_t, ix->n_subvectors, J.nq, q0, ix->metric, lut_ws);
-    TPQ_LAUNCH_CHECK("cell_lut_kernel");
-    const int64_t nt = (int64_t)n * J.n_probe;
-    const int pgrid = (int)((nt + 255) / 256);
-    cell_pairs_count_kernel<<<pgrid, 256, 0, st>>>(J.cells, J.npl, q0, n, J.n_probe, C, ix->cell_start, ix->cell_size,
-                                                   ix->cell_block_start, cell_cnt, slot, ones);
-    TPQ_LAUNCH_CHECK("cell_pairs_count_kernel");
-    ScanArgs A = scan_args(J, q0);
-    A.n_probe_list = ones;
-    qmajor<<<n, 8 * 32, L.total, st>>>(A, L);                              // pass 1: entry 0 of every query
-    TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
-    cell_plan_kernel<<<1, 1024, 0, st>>>(cell_cnt, ix->cell_block_start, ix->cell_size, C, cell_off, items, n_items);
-    TPQ_LAUNCH_CHECK("cell_plan_kernel");
-    cell_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(J.cells, q0, n, J.n_probe, slot, cell_off, pair_q);
-    TPQ_LAUNCH_CHECK("cell_pairs_scatter_kernel");
-    CellArgs CA;
-    CA.codes = ix->codes_scan; CA.valid = ix->block_valid; CA.cell_block_start = ix->cell_block_start;
-    CA.cell_start = ix->cell_start; CA.lut_scan = lut_ws; CA.cell_off = cell_off; CA.cell_cnt = cell_cnt; CA.pair_q = pair_q;
-    CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = J.keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
-    CA.q_base = q0; CA.k = J.k; CA.cap = cap;
-    cscan<<<device_sm_count(), kCellNW * 32, cs_smem, st>>>(CA);
-    TPQ_LAUNCH_CHECK("ivfpq_cell_scan_kernel");
-    cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(J.keys, surv, surv_cnt, q0, n, J.k, kp, cap);
-    TPQ_LAUNCH_CHECK("cell_select_kernel");
-    A.n_probe_list = J.npl; A.only_cnt = surv_cnt; A.only_cap = cap;
-    qmajor<<<n, 8 * 32, L.total, st>>>(A, L);                              // queries whose survivors overflowed
-    TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
-    if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], st);
+    if (prof) cudaEventRecord(g_prof_start[g_prof_n], J.st);
+    if (P.cell_major) {
+      if (int rc = cell_stage(P, J, kern, A, q0, n)) return rc;
+    } else {
+      kern<<<n * P.S, P.NW * 32, P.L.total, J.st>>>(A, P.L);
+      TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
+    }
+    if (prof) cudaEventRecord(g_prof_stop[g_prof_n++], J.st);
   }
   return TPQ_OK;
 }
@@ -1032,76 +1121,11 @@ static int check_index(const tpq_index* ix, int k) {
   return TPQ_OK;
 }
 
-// ws/W: the search workspace, for the cell-major path (nullptr: the fused-push path, which keeps the query-major kernel)
-static int scan_dispatch(const ScanJob& J, uint8_t* ws, const SearchWs* W) {
-  const tpq_index* ix = J.ix;
-  return with_dsub(ix, [&](auto ds) -> int {
-    constexpr int DS = decltype(ds)::value;
-    if constexpr (DS != 0)                                            // cell_major() implies an in-CTA LUT
-      if (ws && !J.n_peers && cell_major(ix, J.S)) return launch_cell_path<DS>(J, ws, *W);
-    if (ix->residual) {
-      // residual IVFPQ.  M <= 64, d/M in {1,2,4}: the query half of the LUT is built into a second shared-memory table (one
-      // 16-warp CTA per SM).  Otherwise it is staged in global memory and added to the per-cell half from L2.
-      if (!ix->part2_scan || !J.base_sims) { set_error("residual search needs part2_scan and base_sims"); return TPQ_ERR_BAD_ARG; }
-      if (ix->metric != TPQ_METRIC_EUCLIDEAN) { set_error("residual IVFPQ is defined for the euclidean metric"); return TPQ_ERR_UNSUPPORTED; }
-#ifdef TPQ_DEBUG_KNOBS
-      { const char* rm = getenv("TPQ_RES_MODE");                    // A/B: staged query half + 3 light CTAs/SM for M <= 64
-        if (rm && !strcmp(rm, "staged3") && ix->m_pad == 64) return launch_scan_d<64, 8, 3, 0, true>(J);
-        if (rm && !strcmp(rm, "staged2") && ix->m_pad == 64) return launch_scan_d<64, 8, 2, 0, true>(J); }
-#endif
-      if constexpr (DS == 1 || DS == 2 || DS == 4)
-        return ix->m_pad == 32 ? launch_scan_d<32, 16, 1, DS, true>(J) : launch_scan_d<64, 16, 1, DS, true>(J);
-      switch (ix->m_pad) {
-        case 32:  return launch_scan_d<32, 16, 1, 0, true>(J);
-        case 64:  return launch_scan_d<64, 16, 1, 0, true>(J);
-        case 96:  return launch_scan_d<96, 16, 1, 0, true>(J);
-        case 128: return launch_scan_d<128, 16, 1, 0, true>(J);
-        case 160: return launch_scan_d<160, 16, 1, 0, true>(J);
-        case 192: return launch_scan_d<192, 16, 1, 0, true>(J);
-        default:
-          set_error("residual IVFPQ: n_subvectors=%d (padded %d) > 192 is not supported", ix->n_subvectors, ix->m_pad);
-          return TPQ_ERR_UNSUPPORTED;
-      }
-    }
-#ifdef TPQ_DEBUG_KNOBS
-    // tuning knob for experiments (scripts/sweep_scan.py): TPQ_SCAN_CFG = "<warps>x<min CTAs/SM>"
-    const char* cfg = getenv("TPQ_SCAN_CFG");
-    if (cfg && ix->m_pad == 64) {
-      if (!strcmp(cfg, "8x2"))  return launch_scan_d<64, 8, 2, DS>(J);
-      if (!strcmp(cfg, "8x3"))  return launch_scan_d<64, 8, 3, DS>(J);
-      if (!strcmp(cfg, "16x1")) return launch_scan_d<64, 16, 1, DS>(J);
-      if (!strcmp(cfg, "4x4"))  return launch_scan_d<64, 4, 4, DS>(J);
-    }
-#endif
-    switch (ix->m_pad) {
-      case 32:  return launch_scan_d<32, 8, 2, DS>(J);
-      case 64: {
-        // Long probe lists: 2 CTAs/SM with a deep prefetch (127 registers).  Short ones (small cells, or one shard of a
-        // cell-sharded index): per-CTA prologue/epilogue weighs more, so 3 lighter CTAs/SM overlap them better.
-        const double blocks_per_cta = (double)ix->n_blocks / ix->n_cells * J.n_probe / J.S;
-        return blocks_per_cta >= 2000.0 ? launch_scan_d<64, 8, 2, DS>(J) : launch_scan_d<64, 8, 3, DS>(J);
-      }
-      case 96:  return launch_scan_d<96, 16, 1, DS>(J);      // LUT >= 128 KB: one CTA per SM, so twice the warps
-      case 128: return launch_scan_d<128, 16, 1, DS>(J);
-      case 160: return launch_scan_d<160, 16, 1, DS>(J);
-      case 192: return launch_scan_d<192, 16, 1, DS>(J);
-      default:
-        set_error("n_subvectors=%d (padded %d) > 192 is not supported by the scan-layout path", ix->n_subvectors, ix->m_pad);
-        return TPQ_ERR_UNSUPPORTED;
-    }
-  });
-}
-
-static int check_ws(const SearchWs& W, const void* ws, size_t ws_bytes) {
-  if (!ws || ws_bytes < W.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, W.total); return TPQ_ERR_WORKSPACE; }
-  return TPQ_OK;
-}
-
 // The coarse stage inside the search workspace: cosine queries are normalised (IVFPQIndex.py:474-475), then every query
 // gets its probe list, the lists' similarities and lengths.
 struct Probes { const float* x; const float* sims; const int64_t* cells; const int64_t* npl; };
 static int coarse_stage(const tpq_index* ix, const float* x_dn, int nq, int n_probe, int smart, float temperature,
-                        uint8_t* w, const SearchWs& W, void* stream, Probes& p) {
+                        uint8_t* w, const SearchWs& W, cudaStream_t stream, Probes& p) {
   p.x = x_dn;
   if (ix->metric == TPQ_METRIC_COSINE) {
     float* xn = reinterpret_cast<float*>(w + W.xnorm);
@@ -1116,14 +1140,34 @@ static int coarse_stage(const tpq_index* ix, const float* x_dn, int nq, int n_pr
   return TPQ_OK;
 }
 
-// scan the batch into the workspace's keys, then merge the slices of every query and decode them
-static int scan_and_merge(const tpq_index* ix, const Probes& p, int nq, int n_probe, int k, uint8_t* w, const SearchWs& W,
-                          float* values, int64_t* ids, int64_t* address, uint64_t* keys_out, cudaStream_t st) {
-  const int S = pick_slices(nq);
-  uint64_t* keys = reinterpret_cast<uint64_t*>(w + W.keys);
-  const ScanJob J{ix, p.x, p.cells, p.npl, p.sims, nq, n_probe, k, S, reinterpret_cast<float*>(w + W.lut), keys, st, nullptr, 0, 0};
-  if (int rc = scan_dispatch(J, w, &W)) return rc;
-  return launch_merge(keys, nq, S, k, k, (int64_t)S * k, ix->address2id, ix->capacity, values, ids, address, keys_out, st);
+// Where a search's keys go: merged across slices and decoded into values / ids / address / keys (each may be null), or,
+// with n_peers > 0, pushed by the scan straight into every peer's gather buffer.
+struct SearchOut {
+  float* values; int64_t* ids; int64_t* address; uint64_t* keys;
+  uint64_t* const* peer_keys; int n_peers, peer_slot;
+};
+
+// The search behind the three entry points, after their argument checks: plan, check the workspace, run the coarse
+// stage unless the probe lists are given (p.cells), scan, then merge or push.
+static int search(const tpq_index* ix, Probes p, int nq, int n_probe, int k, int smart, float temperature,
+                  const SearchOut& o, void* ws, size_t ws_bytes, cudaStream_t st) {
+  const bool push = o.n_peers > 0;
+  const ScanPlan P = plan_scan(ix, nq, n_probe, k, push);
+  if (push && P.S != 1) { set_error("tpq_ivfpq_scan_push: batch of %d queries is sliced; use the gathered exchange", nq); return TPQ_ERR_UNSUPPORTED; }
+  if (push && nq > kQueryChunk) { set_error("tpq_ivfpq_scan_push: at most %d queries per call", kQueryChunk); return TPQ_ERR_UNSUPPORTED; }
+  if (!ws || ws_bytes < P.ws.total) { set_error("workspace too small (%zu < %zu)", ws_bytes, P.ws.total); return TPQ_ERR_WORKSPACE; }
+  if (!p.cells) TPQ_REQUIRE(n_probe <= ix->n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, ix->n_cells);
+  for (int i = 0; i < o.n_peers; ++i) TPQ_REQUIRE(o.peer_keys[i], "null peer buffer");
+  if (ix->residual && (!ix->part2_scan || (p.cells && !p.sims))) { set_error("residual search needs part2_scan and base_sims"); return TPQ_ERR_BAD_ARG; }
+  if (P.rc) { set_error("%s", P.err); return P.rc; }
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  if (!p.cells)
+    if (int rc = coarse_stage(ix, p.x, nq, n_probe, smart, temperature, w, P.ws, st, p)) return rc;
+  if (int rc = launch(P, ScanJob{ix, p.x, p.cells, p.npl, p.sims, nq, n_probe, k, w, st, o.peer_keys, o.n_peers, o.peer_slot}))
+    return rc;
+  if (push) return TPQ_OK;
+  return launch_merge(reinterpret_cast<uint64_t*>(w + P.ws.keys), nq, P.S, k, k, (int64_t)P.S * k, ix->address2id,
+                      ix->capacity, o.values, o.ids, o.address, o.keys, st);
 }
 
 }  // namespace tpq
@@ -1160,7 +1204,7 @@ extern "C" int tpq_profile_scan_ms(float* total_ms, int* n_launches) {
 
 extern "C" size_t tpq_search_workspace_bytes(const tpq_index* ix, int nq, int n_probe, int k) {
   if (!ix || nq <= 0 || n_probe <= 0 || k <= 0) return 0;
-  return search_ws(ix, nq, n_probe, k).total;
+  return plan_scan(ix, nq, n_probe, k, /*push=*/false).ws.total;
 }
 
 extern "C" int tpq_ivfpq_search_cells(const tpq_index* ix, const float* x_dn, const int64_t* cells, const float* base_sims,
@@ -1171,10 +1215,8 @@ extern "C" int tpq_ivfpq_search_cells(const tpq_index* ix, const float* x_dn, co
   TPQ_REQUIRE(nq >= 0 && n_probe >= 1, "bad n_query=%d / n_probe=%d", nq, n_probe);
   TPQ_REQUIRE(x_dn && cells && n_probe_list, "null pointer argument");
   if (nq == 0) return TPQ_OK;
-  const SearchWs W = search_ws(ix, nq, n_probe, k);
-  if (int rc = check_ws(W, ws, ws_bytes)) return rc;
-  return scan_and_merge(ix, Probes{x_dn, base_sims, cells, n_probe_list}, nq, n_probe, k, reinterpret_cast<uint8_t*>(ws), W,
-                        values, ids, address, keys_out, (cudaStream_t)stream);
+  return search(ix, Probes{x_dn, base_sims, cells, n_probe_list}, nq, n_probe, k, 0, 0.f,
+                SearchOut{values, ids, address, keys_out, nullptr, 0, 0}, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int tpq_ivfpq_search(const tpq_index* ix, const float* x_dn, int nq, int n_probe, int k,
@@ -1185,14 +1227,11 @@ extern "C" int tpq_ivfpq_search(const tpq_index* ix, const float* x_dn, int nq, 
   TPQ_REQUIRE(nq >= 0 && x_dn, "bad query batch");
   TPQ_REQUIRE(n_probe >= 1 && n_probe <= ix->n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, ix->n_cells);
   if (nq == 0) return TPQ_OK;
-  const SearchWs W = search_ws(ix, nq, n_probe, k);
-  if (int rc = check_ws(W, ws, ws_bytes)) return rc;
-  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  Probes p;
-  if (int rc = coarse_stage(ix, x_dn, nq, n_probe, smart, temperature, w, W, stream, p)) return rc;
-  return scan_and_merge(ix, p, nq, n_probe, k, w, W, values, ids, address, keys_out, (cudaStream_t)stream);
+  return search(ix, Probes{x_dn, nullptr, nullptr, nullptr}, nq, n_probe, k, smart, temperature,
+                SearchOut{values, ids, address, keys_out, nullptr, 0, 0}, ws, ws_bytes, (cudaStream_t)stream);
 }
 
+// cells == nullptr: the whole coarse stage runs here (replicated probe)
 extern "C" int tpq_ivfpq_scan_push(const tpq_index* ix, const float* x_dn, const int64_t* cells, const float* base_sims,
                                    const int64_t* n_probe_list, int nq, int n_probe, int k, int smart, float temperature,
                                    uint64_t* const* peer_keys, int n_peers, int my_slot,
@@ -1202,20 +1241,9 @@ extern "C" int tpq_ivfpq_scan_push(const tpq_index* ix, const float* x_dn, const
   TPQ_REQUIRE(peer_keys && n_peers >= 1 && n_peers <= 8 && my_slot >= 0, "tpq_ivfpq_scan_push: bad peer list");
   TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "cells and n_probe_list go together");
   if (nq == 0) return TPQ_OK;
-  if (pick_slices(nq) != 1) { set_error("tpq_ivfpq_scan_push: batch of %d queries is sliced; use the gathered exchange", nq); return TPQ_ERR_UNSUPPORTED; }
-  if (nq > kQueryChunk) { set_error("tpq_ivfpq_scan_push: at most %d queries per call", kQueryChunk); return TPQ_ERR_UNSUPPORTED; }
-  const SearchWs W = search_ws(ix, nq, n_probe, k, /*push=*/true);
-  if (int rc = check_ws(W, ws, ws_bytes)) return rc;
-  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  Probes p{x_dn, base_sims, cells, n_probe_list};
-  if (!cells) {                                                       // the whole coarse stage runs here (replicated probe)
-    TPQ_REQUIRE(n_probe <= ix->n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, ix->n_cells);
-    if (int rc = coarse_stage(ix, x_dn, nq, n_probe, smart, temperature, w, W, stream, p)) return rc;
-  }
-  for (int i = 0; i < n_peers; ++i) TPQ_REQUIRE(peer_keys[i], "null peer buffer");
-  const ScanJob J{ix, p.x, p.cells, p.npl, p.sims, nq, n_probe, k, 1, reinterpret_cast<float*>(w + W.lut),
-                  reinterpret_cast<uint64_t*>(w + W.keys), (cudaStream_t)stream, peer_keys, n_peers, my_slot};
-  return scan_dispatch(J, nullptr, nullptr);
+  return search(ix, Probes{x_dn, base_sims, cells, n_probe_list}, nq, n_probe, k, smart, temperature,
+                SearchOut{nullptr, nullptr, nullptr, nullptr, peer_keys, n_peers, my_slot}, ws, ws_bytes,
+                (cudaStream_t)stream);
 }
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k,

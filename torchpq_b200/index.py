@@ -273,36 +273,38 @@ class IVFPQIndex(StateModule):
         assert x.dtype == torch.float32 and x.device == self._address2id.device
         return x.contiguous()
 
+    def _search(self, x, k, n_probe, call, outputs=True, return_address=False, return_keys=False):
+        """The body of search, search_cells and scan_push: allocates the outputs (values, ids and those the flags ask
+        for; none for scan_push) and the workspace tpq_search_workspace_bytes asks for, then runs
+        call(index, values, ids, address, keys, ws, ws_bytes, stream) on their pointers."""
+        lay = self.layout()
+        dev, nq = x.device, x.shape[1]
+        new = lambda dtype: torch.empty(nq, k, dtype=dtype, device=dev)
+        values, ids = (new(torch.float32), new(torch.long)) if outputs else (None, None)
+        address = new(torch.long) if return_address else None
+        keys = new(torch.int64) if return_keys else None
+        out = ((values, ids) + ((address,) if return_address else ()) + ((keys,) if return_keys else ())) if outputs else None
+        if nq == 0 and outputs:                                        # an empty batch has no storage to point at
+            return out
+        ws_bytes = lib.tpq_search_workspace_bytes(C.byref(lay.cindex), nq, n_probe, k)
+        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
+        check(call(C.byref(lay.cindex), ptr(values), ptr(ids), ptr(address), ptr(keys), ptr(ws), ws_bytes,
+                   _lib.current_stream(dev)))
+        return out
+
     def search(self, x, k=1, return_address=False, return_keys=False):
         """IVFPQIndex.search (IVFPQIndex.py:469-524): x [d_vector, n_query] fp32 on the index device
         -> (topk_values [n_query, k] fp32 descending, topk_ids [n_query, k] int64[, topk_address])."""
         x = self._check_query(x, k)
-        lay = self.layout()
-        dev, nq = x.device, x.shape[1]
-        values = torch.empty(nq, k, dtype=torch.float32, device=dev)
-        ids = torch.empty(nq, k, dtype=torch.long, device=dev)
-        address = torch.empty(nq, k, dtype=torch.long, device=dev) if return_address else None
-        keys = torch.empty(nq, k, dtype=torch.int64, device=dev) if return_keys else None
-        if nq == 0:                                                    # an empty batch has no storage to point at
-            return (values, ids) + ((address,) if return_address else ()) + ((keys,) if return_keys else ())
         n_probe = int(self.n_probe)
-        ws_bytes = lib.tpq_search_workspace_bytes(C.byref(lay.cindex), nq, n_probe, k)
-        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
-        check(lib.tpq_ivfpq_search(C.byref(lay.cindex), ptr(x), nq, n_probe, k,
-                                   int(bool(self.use_smart_probing)), float(self.smart_probing_temperature),
-                                   ptr(values), ptr(ids), ptr(address), ptr(keys), ptr(ws), ws_bytes,
-                                   _lib.current_stream(dev)))
-        out = (values, ids)
-        if return_address:
-            out = out + (address,)
-        if return_keys:
-            out = out + (keys,)
-        return out
+        smart, temperature = int(bool(self.use_smart_probing)), float(self.smart_probing_temperature)
+        return self._search(x, k, n_probe, lambda ix, *out: lib.tpq_ivfpq_search(ix, ptr(x), x.shape[1], n_probe, k, smart,
+                                                                                  temperature, *out),
+                            return_address=return_address, return_keys=return_keys)
 
     def search_cells(self, x, cells, base_sims=None, n_probe_list=None, k=1, return_address=False, return_keys=False):
         """IVFPQIndex.search_cells, non-residual branch (IVFPQIndex.py:407-467)."""
         x = self._check_query(x, k)
-        lay = self.layout()
         dev, nq = x.device, x.shape[1]
         assert cells.dtype == torch.int64 and cells.shape[0] == nq and cells.dim() == 2
         n_probe = cells.shape[1]
@@ -310,47 +312,31 @@ class IVFPQIndex(StateModule):
             n_probe_list = torch.zeros(nq, dtype=torch.long, device=dev) + n_probe
         assert n_probe_list.shape == (nq,) and n_probe_list.dtype == torch.int64     # IVFPQTopkCuda.py:109-110
         cells, n_probe_list = cells.contiguous(), n_probe_list.contiguous()
-        values = torch.empty(nq, k, dtype=torch.float32, device=dev)
-        ids = torch.empty(nq, k, dtype=torch.long, device=dev)
-        address = torch.empty(nq, k, dtype=torch.long, device=dev) if return_address else None
-        keys = torch.empty(nq, k, dtype=torch.int64, device=dev) if return_keys else None
-        if nq == 0:
-            return (values, ids) + ((address,) if return_address else ()) + ((keys,) if return_keys else ())
-        ws_bytes = lib.tpq_search_workspace_bytes(C.byref(lay.cindex), nq, n_probe, k)
-        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
-        if self.pq_use_residual:
+        if not self.pq_use_residual:
+            base_sims = None
+        elif nq > 0:
             assert base_sims is not None, "base_sims is required when pq_use_residual is True"   # IVFPQIndex.py:424
             assert base_sims.shape == (nq, n_probe) and base_sims.dtype == torch.float32
             base_sims = base_sims.contiguous()
-        check(lib.tpq_ivfpq_search_cells(C.byref(lay.cindex), ptr(x), ptr(cells),
-                                         ptr(base_sims if self.pq_use_residual else None), ptr(n_probe_list), nq, n_probe, k,
-                                         ptr(values), ptr(ids), ptr(address), ptr(keys), ptr(ws), ws_bytes,
-                                         _lib.current_stream(dev)))
-        out = (values, ids)
-        if return_address:
-            out = out + (address,)
-        if return_keys:
-            out = out + (keys,)
-        return out
+        return self._search(x, k, n_probe, lambda ix, *out: lib.tpq_ivfpq_search_cells(ix, ptr(x), ptr(cells), ptr(base_sims),
+                                                                                        ptr(n_probe_list), nq, n_probe, k, *out),
+                            return_address=return_address, return_keys=return_keys)
 
     def scan_push(self, x, k, peer_ptrs, n_peers, my_slot, cells=None, base_sims=None, n_probe_list=None):
         """The scan of search / search_cells with its output fused into the cross-shard exchange (tpq_ivfpq_scan_push):
         every CTA stores its top-k keys into slot `my_slot` of each rank's gather buffer (`peer_ptrs`: a ctypes array of
         device pointers into peer-mapped memory).  Raises NotImplementedError for batches small enough to be sliced."""
         x = self._check_query(x, k)
-        lay = self.layout()
-        dev, nq = x.device, x.shape[1]
         n_probe = int(self.n_probe) if cells is None else cells.shape[1]
         if cells is not None:
-            assert cells.dtype == torch.int64 and cells.shape[0] == nq and n_probe_list is not None
+            assert cells.dtype == torch.int64 and cells.shape[0] == x.shape[1] and n_probe_list is not None
             cells, n_probe_list = cells.contiguous(), n_probe_list.contiguous()
             base_sims = base_sims.contiguous() if base_sims is not None else None
             assert not self.pq_use_residual or base_sims is not None
-        ws_bytes = lib.tpq_search_workspace_bytes(C.byref(lay.cindex), nq, n_probe, k)
-        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
-        check(lib.tpq_ivfpq_scan_push(C.byref(lay.cindex), ptr(x), ptr(cells), ptr(base_sims), ptr(n_probe_list), nq, n_probe, k,
-                                      int(bool(self.use_smart_probing)), float(self.smart_probing_temperature),
-                                      peer_ptrs, n_peers, my_slot, ptr(ws), ws_bytes, _lib.current_stream(dev)))
+        smart, temperature = int(bool(self.use_smart_probing)), float(self.smart_probing_temperature)
+        self._search(x, k, n_probe, lambda ix, _v, _i, _a, _k, *ws: lib.tpq_ivfpq_scan_push(
+            ix, ptr(x), ptr(cells), ptr(base_sims), ptr(n_probe_list), x.shape[1], n_probe, k, smart, temperature,
+            peer_ptrs, n_peers, my_slot, *ws), outputs=False)
 
     # ------------------------------------------------------------------ build side (see build.py)
     def train(self, x, force_retrain=False, seed=0):

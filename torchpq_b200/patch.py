@@ -14,7 +14,7 @@ import types
 
 from .index import IVFPQIndex as _Mine
 
-_METHODS = ("layout", "set_shard", "_check_query", "search", "search_cells")
+_METHODS = ("layout", "set_shard", "_check_query", "_search", "search", "search_cells")
 
 
 def patch(index):
