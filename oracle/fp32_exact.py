@@ -145,8 +145,8 @@ def _split(x, M):
 
 
 def lut_entries(x, pq, kind):
-    """One LUT entry per (m, q, code), the arithmetic shared by build_lut_kernel (lut.cu:24-41), lut_scan_kernel
-    (scan.cu:55-88), build_lut (scan.cu:311-345) and so cell_lut_kernel (scan.cu:749-753): dot = fmaf chain of
+    """One LUT entry per (m, q, code), the arithmetic of lut.cuh:23-35 that lut_kernel (lut.cu:18-68), build_lut
+    (lut.cuh:40-79) and so cell_lut_kernel (scan.cu:654-659) share: dot = fmaf chain of
     x_m[i] * p_m[i][code] over i ascending from +0; |x_m|^2 and |p|^2 are sums of separately rounded squares;
     kind "euclidean": ((dot * 2) - |x_m|^2) - |p|^2; "cosine": dot; "part1" (residual query half): dot * 2.
     x [d, nq], pq [M, dsub, 256] -> [M, nq, 256]."""
@@ -165,14 +165,14 @@ def lut_entries(x, pq, kind):
 
 
 def build_lut(x, pq, distance):
-    """build_lut_kernel (lut.cu:18-43), the reference-layout LUT of tpq_build_lut / fn.precompute_adc: [M, nq, 256]."""
+    """lut_kernel in the reference layout (lut.cu:65), the LUT of tpq_build_lut / fn.precompute_adc: [M, nq, 256]."""
     return lut_entries(x, pq, distance)
 
 
 def lut_scan(x, pq, distance, residual=False):
     """The LUT in scan layout (scan_layout.cuh:17-18), per query and sub-quantizer: [nq, m_pad, 256], the rows of
-    padding sub-quantizers m >= M +0 (lut_scan_kernel :83-89; build_lut reads zero sub-vectors and a zero-padded
-    codebook, relayout.cu:76).  residual: the query half part1 = dot * 2 (scan.cu:87, :343)."""
+    padding sub-quantizers m >= M +0 (lut_kernel, lut.cu:64-65; build_lut reads zero sub-vectors and a zero-padded
+    codebook, relayout.cu:76).  residual: the query half part1 = dot * 2 (lut.cuh:32)."""
     pq = np.asarray(pq, F32)
     M = pq.shape[0]
     mp = (M + 31) // 32 * 32
@@ -183,8 +183,9 @@ def lut_scan(x, pq, distance, residual=False):
 
 
 def part2(vq, pq):
-    """relayout_part2_kernel (relayout.cu:85-105): part2[c, m, code] = (dot * -2) - nrm * nrm, dot = fmaf chain of
-    vq[m * dsub + i, c] * pq[m, i, code], nrm = sqrtf(fmaf chain of pq[m, i, code]^2), i ascending from +0;
+    """tpq_relayout_part2 (relayout.cu:91-101: lut_kernel, kind part 2, lut.cuh:27, :33): part2[c, m, code] =
+    (dot * -2) - nrm * nrm, dot = fmaf chain of vq[m * dsub + i, c] * pq[m, i, code], nrm = sqrtf(fmaf chain of
+    pq[m, i, code]^2), i ascending from +0;
     padding sub-quantizers +0.  vq [d, C], pq [M, dsub, 256] -> [C, m_pad, 256]."""
     pq = np.asarray(pq, F32)
     M, dsub, _ = pq.shape
@@ -207,8 +208,8 @@ def rot_subq(t, lane):
 
 
 def scan_scores(st, lut, addr, lane, base=F32(0)):
-    """The score one scan lane forms for each address (adc_unit scan.cu:134-143, process_block :184-188,
-    key_of_block :201-208, the cell-major kernel :714-716): record byte t of lane l holds sub-quantizer rot_subq(t, l)
+    """The score one scan lane forms for each address (adc_unit scan.cu:73-82, process_block :123-127,
+    key_of_block :140-147, the cell-major kernel :614-616): record byte t of lane l holds sub-quantizer rot_subq(t, l)
     (code 0 for padding); acc[J] sums the LUT entries of record bytes t = J, J + 4, ... in ascending t from +0 (a
     64-sub-quantizer unit at a time; at m_pad 96 the last unit is 32 bytes, the same ascending t);
     score = base + ((acc0 + acc1) + (acc2 + acc3)).
@@ -233,7 +234,7 @@ def _cell_lanes(st, addr):
 
 
 def search_cells_fp32(st, x, cells, n_probe_list, k, base_sims=None, residual=False, part2_table=None):
-    """tpq_ivfpq_search_cells (scan.cu:1153-1165): the scan of caller-supplied probe lists, in the kernels' own
+    """tpq_ivfpq_search_cells (scan.cu:1100-1110): the scan of caller-supplied probe lists, in the kernels' own
     arithmetic.  x [d, nq] is used as given (no cosine normalisation, as there); the visiting rule is the oracle's
     (plain: O.effective_probes / O.probed_addresses; residual: P = clip((int) n_probe_list, 0, n_probe), entries whose
     start equals the previous entry's skipped, ivfpq_topk.cu:1080-1104), the selection O.select_topk.
@@ -267,7 +268,7 @@ def search_cells_fp32(st, x, cells, n_probe_list, k, base_sims=None, residual=Fa
             prev = s
             a = np.arange(s, s + n, dtype=np.int64)
             a = a[live[a]]
-            lut = (luts[q] + p2[c]).astype(F32)                 # store_precomputed_to_smem: part1 + part2 (scan.cu:450-453)
+            lut = (luts[q] + p2[c]).astype(F32)                 # store_precomputed_to_smem: part1 + part2 (scan.cu:343-346)
             sc.append(scan_scores(st, lut, a, (a - s) & 31, base[q, j]))
             ad.append(a)
         vals[q], adr[q] = O.select_topk(np.concatenate(sc), np.concatenate(ad), k)
@@ -275,7 +276,7 @@ def search_cells_fp32(st, x, cells, n_probe_list, k, base_sims=None, residual=Fa
 
 
 def search_fp32(st, x, k, residual=False, n_probe_list=None):
-    """tpq_ivfpq_search (scan.cu:1167-1181) in the kernels' arithmetic: cosine queries normalised (normalize_columns),
+    """tpq_ivfpq_search (scan.cu:1112-1122) in the kernels' arithmetic: cosine queries normalised (normalize_columns),
     coarse probe (coarse_sims + probe_select), then search_cells_fp32 with the probe similarities as the residual
     base.  n_probe_list: the per-query list lengths; None = n_probe without smart probing, else the oracle's smart
     probing of the restated probe similarities (not bit-exact: pass the GPU's own list to pin bits).

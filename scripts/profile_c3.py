@@ -26,7 +26,7 @@ import bench  # noqa: E402
 # kernels launched inside the scan stage's profiling events (tpq_profile_*): the query-major scan, or the cell-major
 # path's LUTs, pair list, plan, pass 1, cell scan, select and re-run
 SCAN_STAGE = ("ivfpq_scan_kernel", "ivfpq_cell_scan_kernel", "cell_lut_kernel", "cell_pairs_count_kernel",
-              "cell_pairs_scatter_kernel", "cell_plan_kernel", "cell_select_kernel", "lut_scan_kernel")
+              "cell_pairs_scatter_kernel", "cell_plan_kernel", "cell_select_kernel", "lut_kernel")
 
 
 def short_name(name):

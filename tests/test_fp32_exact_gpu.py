@@ -120,9 +120,33 @@ def test_precompute_adc(cuda_device, M, dsub):
             assert_bits(got, X.build_lut(x, pq, distance))
 
 
+@pytest.mark.parametrize("M,dsub", [(8, 128), (4, 460), (1, 7300)])
+def test_precompute_adc_wide(cuda_device, M, dsub):
+    """Wide sub-vectors: lut_kernel's shared-memory tile above 48 KB (128), with fewer sub-quantizers per CTA (460), and
+    with one query and one sub-quantizer per CTA (7300)."""
+    import torchpq_b200 as T
+    pq = _randn((M, dsub, 256), M + dsub)
+    x = _randn((M * dsub, 17), dsub)
+    for distance in ("euclidean", "cosine"):
+        assert_bits(T.fn.precompute_adc(g(x), g(pq), distance).cpu().numpy(), X.build_lut(x, pq, distance))
+
+
+@pytest.mark.parametrize("M", [8, 64, 120])
+@pytest.mark.parametrize("dsub", [1, 2, 3])
+def test_part2_scan(cuda_device, M, dsub):
+    """The residual index's per-cell half of the LUT (ScanLayout.part2_scan) in scan layout: the m_pad rows equal their
+    restatement, and the rest of a partly used last 64-sub-quantizer group is +0."""
+    st = B.randn_state(M * dsub, M, 50, 1000, seed=M + dsub)
+    lay = make_residual_index(st).layout()
+    mp, mg = lay.m_pad, (lay.m_pad + 63) // 64
+    got = lay.part2_scan.view(st.n_cells, mg, 256, 64).transpose(2, 3).reshape(st.n_cells, mg * 64, 256).cpu().numpy()
+    assert_bits(got[:, :mp], X.part2(st.vq_codebook, st.pq_codebook))
+    assert not got[:, mp:].view(np.uint32).any()
+
+
 @pytest.mark.parametrize("nq", [15, 16, 1000])
 def test_precompute_adc_query_tiles(cuda_device, nq):
-    """Query counts around build_lut_kernel's 16-query CTA tile."""
+    """Query counts around and across the LUT kernel's query tiles."""
     import torchpq_b200 as T
     pq = _randn((8, 3, 256), 9)
     x = _randn((24, nq), nq)
@@ -236,7 +260,7 @@ def test_search_in_cta_lut(cuda_device, dsub):
     run_search(st, _randn((16 * dsub, 64), dsub), 50, m_pad=32, staged=False)
 
 
-@pytest.mark.parametrize("dsub", [3, 12])
+@pytest.mark.parametrize("dsub", [3, 12, 96, 128])
 def test_search_staged_lut(cuda_device, dsub):
     st = B.randn_state(16 * dsub, 16, 24, 6000, seed=dsub)
     st.n_probe = 6

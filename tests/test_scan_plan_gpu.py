@@ -73,9 +73,9 @@ def test_m32(cuda_device):
 
 
 def test_m96_staged_lut(cuda_device):
-    """d/M = 3 has no in-CTA LUT build: lut_scan_kernel stages it"""
+    """d/M = 3 has no in-CTA LUT build: lut_kernel stages it"""
     ix, queries = index_of(288, 96, 3000, 4)
-    assert searched(ix, queries, NQ) == {"lut_scan_kernel", "ivfpq_scan_kernel<96, 16, 1, 0, false>", "merge_topk_kernel"}
+    assert searched(ix, queries, NQ) == {"lut_kernel<0, 1>", "ivfpq_scan_kernel<96, 16, 1, 0, false>", "merge_topk_kernel"}
 
 
 def test_m120_cosine(cuda_device):
@@ -85,8 +85,8 @@ def test_m120_cosine(cuda_device):
 
 @pytest.mark.parametrize("d, M, want", [
     (128, 64, {"ivfpq_scan_kernel<64, 16, 1, 2, true>"}),
-    (512, 64, {"lut_scan_kernel", "ivfpq_scan_kernel<64, 16, 1, 0, true>"}),
-    (192, 96, {"lut_scan_kernel", "ivfpq_scan_kernel<96, 16, 1, 0, true>"}),
+    (512, 64, {"lut_kernel<2, 1>", "ivfpq_scan_kernel<64, 16, 1, 0, true>"}),
+    (192, 96, {"lut_kernel<2, 1>", "ivfpq_scan_kernel<96, 16, 1, 0, true>"}),
 ])
 def test_residual(cuda_device, d, M, want):
     ix, queries = index_of(d, M, 3000, 4, residual=True)

@@ -1,5 +1,5 @@
 // Builds the scan layout (format: scan_layout.cuh) and the scan-side codebooks from the reference's buffers.
-#include "scan_layout.cuh"
+#include "lut.cuh"
 
 namespace tpq {
 
@@ -80,30 +80,6 @@ __global__ void relayout_codebook_kernel(const float* __restrict__ cb, int M, in
   nrm[idx] = (metric == TPQ_METRIC_EUCLIDEAN) ? b2 : 0.f;
 }
 
-// part2_scan[c][g][code][s] = -2 * sum_i vq[(64g+s)*dsub + i][c] * pq[64g+s][i][code] - (||p||)^2, zero for padding
-// sub-quantizers.  ||p||^2 is formed as norm * norm, the way the reference's `.norm(dim=1).pow(2)` does (IVFPQIndex.py:167-170).
-__global__ void __launch_bounds__(256)
-relayout_part2_kernel(const float* __restrict__ vq, const float* __restrict__ pq, int M, int MP, int dsub, int C,
-                      float* __restrict__ out) {
-  const int c = blockIdx.x, code = threadIdx.x;
-  const int MG = lut_groups(MP);
-  float* o = out + (size_t)c * MG * kLutGroup;
-  for (int m = 0; m < MG * 64; ++m) {
-    float y = 0.f;
-    if (m < M) {
-      float dot = 0.f, n2 = 0.f;
-      for (int i = 0; i < dsub; ++i) {
-        const float pv = pq[((size_t)m * dsub + i) * 256 + code];
-        dot = fmaf(vq[(size_t)(m * dsub + i) * C + c], pv, dot);
-        n2 = fmaf(pv, pv, n2);
-      }
-      const float nrm = sqrtf(n2);
-      y = __fsub_rn(__fmul_rn(dot, -2.f), __fmul_rn(nrm, nrm));
-    }
-    o[lut_index(m, code)] = y;
-  }
-}
-
 }  // namespace tpq
 
 using namespace tpq;
@@ -116,10 +92,12 @@ extern "C" int tpq_relayout_part2(const float* vq_codebook, const float* pq_code
                                   float* part2_scan, void* stream) {
   TPQ_REQUIRE(vq_codebook && pq_codebook && part2_scan, "tpq_relayout_part2: null pointer");
   TPQ_REQUIRE(d > 0 && M > 0 && d % M == 0 && n_cells > 0, "tpq_relayout_part2: bad sizes");
-  const int MP = scan_m_pad(M);
-  relayout_part2_kernel<<<n_cells, 256, 0, (cudaStream_t)stream>>>(vq_codebook, pq_codebook, M, MP, d / M, n_cells, part2_scan);
-  TPQ_LAUNCH_CHECK("relayout_part2_kernel");
-  return TPQ_OK;
+  // part2_scan[c] = the residual LUT's cell half (lut.cuh), the cells of vq_codebook [d, n_cells] as the rows.  The
+  // kernel writes m_pad rows; a partly used last group's other rows stay +0.
+  if (scan_m_pad(M) % 64)
+    TPQ_CUDA(cudaMemsetAsync(part2_scan, 0, tpq_part2_scan_bytes(M, n_cells), (cudaStream_t)stream));
+  return launch_lut(vq_codebook, n_cells, 0, n_cells, pq_codebook, d, M, kLutPart2, kLutScan, part2_scan,
+                    (cudaStream_t)stream);
 }
 
 extern "C" int tpq_relayout_plan(const int64_t* cell_size, int n_cells, int shard_rank, int shard_world,

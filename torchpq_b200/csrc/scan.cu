@@ -10,8 +10,8 @@
 //   * one PRMT builds the whole address: byte 1 = the code byte, byte 0 = the lane's
 //     precomputed slot offset, bytes 2..3 = sign-replicated zero; the half-group and
 //     group offsets are LDS immediates.  Inner loop = PRMT + LDS + FADD per code byte.
-//   * the LUT itself is built by the CTA, in place, from the L2-resident transposed codebook (d/M in
-//     {1,2,4}; otherwise it is staged through HBM by lut_scan_kernel).
+//   * the LUT itself is built by the CTA, in place, from the L2-resident transposed codebook (build_lut, lut.cuh; d/M
+//     in {1,2,4,8}); otherwise it is staged through HBM by lut_kernel (lut.cu).
 //   * each warp streams whole 32-vector blocks with coalesced 128-bit loads in units of 64
 //     sub-quantizers, software pipelined one unit ahead (ping-pong register sets).
 //   * top-k (CtaTopK, common.cuh): one compare against the CTA-wide running k-th best + one ballot per
@@ -25,71 +25,10 @@
 #include <stdlib.h>
 #include <string.h>
 #include <type_traits>
-#include "scan_layout.cuh"
+#include "lut.cuh"
 #include "tc_common.cuh"
 
 namespace tpq {
-
-// ----------------------------------------------------------------------------- LUT in scan layout (global)
-// lut_scan[q][g][code][s] = LUT[64 g + s][q][code], zero for padding sub-quantizers.  Same arithmetic as lut.cu
-// (PQCodec.py:62-75, MultiKMeans.py:183-223).  Used when d/M is too large for the in-CTA build.
-// CTA = 256 codes x 16 sub-quantizers x LS_QT queries: every codebook value is loaded once (coalesced over the
-// code) and reused for LS_QT queries; query sub-vectors are broadcast from shared memory.
-constexpr int LS_QT = 8, LS_MT = 16;
-constexpr int kLutPart1 = 2;          // lut_scan_kernel `metric` value: the query half of the residual LUT
-__global__ void __launch_bounds__(256)
-lut_scan_kernel(const float* __restrict__ x, const float* __restrict__ cb, int d, int M, int MP, int nq,
-                int q_base, int n_chunk, int metric, float* __restrict__ lut_scan) {
-  extern __shared__ __align__(16) float xs[];            // [LS_QT][LS_MT * dsub] sub-vectors, then [LS_QT][LS_MT] |x_m|^2
-  const int dsub = d / M;
-  const int m0 = blockIdx.y * LS_MT;
-  const int q0 = blockIdx.x * LS_QT;                     // within this chunk
-  const int c = threadIdx.x;
-  float* a2s = xs + LS_QT * LS_MT * dsub;
-  for (int i = threadIdx.x; i < LS_QT * LS_MT * dsub; i += blockDim.x) {
-    const int qq = i / (LS_MT * dsub), r = i % (LS_MT * dsub);
-    const int row = m0 * dsub + r;
-    xs[i] = (q0 + qq < n_chunk && row < d) ? x[(size_t)row * nq + q_base + q0 + qq] : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < LS_QT * LS_MT; i += blockDim.x) {
-    const float* v = xs + (size_t)i * dsub;
-    float a2 = 0.f;
-    for (int e = 0; e < dsub; ++e) a2 = __fadd_rn(a2, __fmul_rn(v[e], v[e]));
-    a2s[i] = a2;
-  }
-  __syncthreads();
-  const int MG = lut_groups(MP);
-  for (int mm = 0; mm < LS_MT; ++mm) {
-    const int m = m0 + mm;
-    if (m >= MP) break;
-    float dot[LS_QT];
-    #pragma unroll
-    for (int qq = 0; qq < LS_QT; ++qq) dot[qq] = 0.f;
-    float b2 = 0.f;
-    if (m < M) {
-      const float* p = cb + (size_t)m * dsub * 256 + c;
-      #pragma unroll 4
-      for (int e = 0; e < dsub; ++e) {
-        const float pv = __ldg(p + (size_t)e * 256);
-        b2 = __fadd_rn(b2, __fmul_rn(pv, pv));
-        #pragma unroll
-        for (int qq = 0; qq < LS_QT; ++qq) dot[qq] = fmaf(xs[(qq * LS_MT + mm) * dsub + e], pv, dot[qq]);
-      }
-    }
-    #pragma unroll
-    for (int qq = 0; qq < LS_QT; ++qq) {
-      if (q0 + qq >= n_chunk) break;
-      float y = 0.f;
-      if (m < M) {
-        y = dot[qq];
-        if (metric == TPQ_METRIC_EUCLIDEAN) y = __fsub_rn(__fsub_rn(__fmul_rn(dot[qq], 2.f), a2s[qq * LS_MT + mm]), b2);
-        else if (metric == kLutPart1) y = __fmul_rn(dot[qq], 2.f);   // residual IVFPQ: part1 = 2 <x_m, p> (IVFPQIndex.py:377)
-      }
-      lut_scan[(size_t)(q0 + qq) * MG * kLutGroup + lut_index(m, c)] = y;
-    }
-  }
-}
 
 // ----------------------------------------------------------------------------- scan kernel
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
@@ -301,54 +240,8 @@ __device__ __forceinline__ void write_keys(const ScanArgs& A, const uint64_t* li
   for (int i = tid; i < A.k; i += NW * 32) out[i] = list[i];
 }
 
-// The LUT of query q in scan layout (RES: the query half of the residual LUT), built by the NW warps of a CTA
-// (PQCodec.py:62-75; MultiKMeans.py:183-223; same arithmetic as lut.cu).  Lane l owns sub-quantizers m = 32 h + l: reads
-// of the transposed codebook are contiguous across the warp, and so is every store (128 B), in shared or global memory.
-template <int MP, int NW, int DSUB, bool RES>
-__device__ __forceinline__ void build_lut(float* lutf, const float* __restrict__ x, const float* __restrict__ cbt, int M,
-                                          int nq, int q, int metric, int lane, int warp) {
-  constexpr int NH = MP / 32;
-  float xr[NH][DSUB], a2[NH];
-  #pragma unroll
-  for (int h = 0; h < NH; ++h) {
-    const int m = 32 * h + lane;
-    float s2 = 0.f;
-    #pragma unroll
-    for (int i = 0; i < DSUB; ++i) {
-      const float v = (m < M) ? __ldg(x + (size_t)(m * DSUB + i) * nq + q) : 0.f;
-      xr[h][i] = v;
-      s2 = __fadd_rn(s2, __fmul_rn(v, v));
-    }
-    a2[h] = s2;
-  }
-  #pragma unroll (DSUB >= 8 ? 2 : 8)
-  for (int c = warp; c < 256; c += NW) {
-    #pragma unroll
-    for (int h = 0; h < NH; ++h) {
-      const float* p = cbt + ((size_t)c * MP + 32 * h + lane) * DSUB;
-      float pv[DSUB];
-      if constexpr (DSUB == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); pv[0] = t.x; pv[1] = t.y; }
-      else if constexpr (DSUB % 4 == 0) {
-        #pragma unroll
-        for (int i = 0; i < DSUB; i += 4) {
-          const float4 t = __ldg(reinterpret_cast<const float4*>(p + i));
-          pv[i] = t.x; pv[i + 1] = t.y; pv[i + 2] = t.z; pv[i + 3] = t.w;
-        }
-      }
-      else { for (int i = 0; i < DSUB; ++i) pv[i] = __ldg(p + i); }
-      float dot = 0.f, b2 = 0.f;
-      #pragma unroll
-      for (int i = 0; i < DSUB; ++i) { dot = fmaf(xr[h][i], pv[i], dot); b2 = __fadd_rn(b2, __fmul_rn(pv[i], pv[i])); }
-      float y = dot;
-      if constexpr (RES) y = __fmul_rn(dot, 2.f);                    // part1 = 2 <x_m, p> (IVFPQIndex.py:377)
-      else if (metric == TPQ_METRIC_EUCLIDEAN) y = __fsub_rn(__fsub_rn(__fmul_rn(dot, 2.f), a2[h]), b2);
-      lutf[lut_index(32 * h + lane, c)] = y;
-    }
-  }
-}
-
-// DSUB > 0: the CTA builds its query's LUT itself from the (L2-resident) transposed codebook -- no LUT
-// round trip through HBM, no LUT workspace.  DSUB == 0: the LUT was written by lut_scan_kernel and is copied in.
+// DSUB > 0: the CTA builds its query's LUT itself (build_lut, lut.cuh) from the (L2-resident) transposed codebook -- no
+// LUT round trip through HBM, no LUT workspace.  DSUB == 0: the LUT was staged by lut_kernel (lut.cu) and is copied in.
 // RES: residual IVFPQ (ivfpq_topk_residual_precomputed, ivfpq_topk.cu:1039-1207).  The LUT of a (query, cell) pair
 // is part1[query] + part2[cell]: the query half is built once into a second shared-memory table, and the CTA
 // walks the probed cells in lock step, re-forming the LUT (one float4 add per 16 bytes) before each cell; the
@@ -823,7 +716,7 @@ struct ScanPlan {
   int S, chunk;                   // CTAs (slices) per query; queries per scan launch
   bool cell_major;                // the cell-major stage (ivfpq_cell_scan_kernel) instead of one query-major launch
   int dsub;                       // LUT source: d/M = 1, 2, 4 or 8 when built in the kernel (on the cell-major path:
-                                  // by cell_lut_kernel), 0 = staged through global memory by lut_scan_kernel
+                                  // by cell_lut_kernel), 0 = staged through global memory by lut_kernel
   bool residual, part1_in_smem;   // residual IVFPQ; its query half of the LUT in a second shared-memory table
   int MP, NW, MINB;               // the query-major kernel: ivfpq_scan_kernel<MP, NW, MINB, qm_dsub(), residual>
   int boot_r;                     // blocks per warp in the kernel's bootstrap
@@ -873,7 +766,7 @@ static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool 
   P.boot_r = 2;
   // LUT source: built inside the scan CTA when d/M is 1, 2, 4 or 8 (the codebook slice a CTA reads from L2, M*dsub KB,
   // is then small next to the codes it goes on to stream: C4, d/M = 8, reads 0.98 MB of codebook per 7.5 MB of codes
-  // and saves the 2 x 128 KB LUT round trip through HBM plus one launch); staged through HBM by lut_scan_kernel
+  // and saves the 2 x 128 KB LUT round trip through HBM plus one launch); staged through HBM by lut_kernel
   // otherwise.  Residual IVFPQ keeps TWO tables when the query half is built in the CTA: that fits for M <= 64 and pays
   // for d/M <= 4.
   P.dsub = (dsub == 1 || dsub == 2 || dsub == 4 || dsub == 8) ? dsub : 0;
@@ -891,9 +784,9 @@ static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool 
   }
 #ifdef TPQ_DEBUG_KNOBS
   // experiment knobs (scripts/sweep_scan.py), read once per search
-  const char* lm = getenv("TPQ_LUT_MODE");            // "staged": every LUT through lut_scan_kernel
+  const char* lm = getenv("TPQ_LUT_MODE");            // "staged": every LUT through lut_kernel
   if (lm && !strcmp(lm, "staged")) P.dsub = 0;
-  const char* rm = getenv("TPQ_RES_MODE");            // residual, "staged*": the query half through lut_scan_kernel,
+  const char* rm = getenv("TPQ_RES_MODE");            // residual, "staged*": the query half through lut_kernel,
   if (P.residual && rm && !strncmp(rm, "staged", 6)) {  // "staged2|3": with 8-warp CTAs, 2|3 per SM, at M <= 64
     P.dsub = 0;
     if (P.MP == 64 && !strcmp(rm, "staged3")) { P.NW = 8; P.MINB = 3; }
@@ -1083,12 +976,9 @@ static int launch(const ScanPlan& P, const ScanJob& J) {
   for (int q0 = 0; q0 < J.nq; q0 += P.chunk) {
     const int n = (J.nq - q0) < P.chunk ? (J.nq - q0) : P.chunk;
     if (!P.cell_major && P.dsub == 0) {
-      const size_t xs_bytes = (size_t)LS_QT * LS_MT * (ix->d_vector / ix->n_subvectors + 1) * 4;
-      dim3 lgrid((n + LS_QT - 1) / LS_QT, (P.MP + LS_MT - 1) / LS_MT);
-      lut_scan_kernel<<<lgrid, 256, xs_bytes, J.st>>>(J.x, ix->pq_codebook, ix->d_vector, ix->n_subvectors, P.MP, J.nq,
-                                                      q0, n, P.residual ? kLutPart1 : ix->metric,
-                                                      reinterpret_cast<float*>(J.w + P.ws.lut));
-      TPQ_LAUNCH_CHECK("lut_scan_kernel");
+      if (int rc = launch_lut(J.x, J.nq, q0, n, ix->pq_codebook, ix->d_vector, ix->n_subvectors,
+                              P.residual ? kLutPart1 : ix->metric, kLutScan, reinterpret_cast<float*>(J.w + P.ws.lut), J.st))
+        return rc;
     }
     const ScanArgs A = scan_args(P, J, q0);
     const bool prof = g_prof_on && g_prof_n < kProfMax;
