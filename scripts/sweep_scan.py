@@ -2,8 +2,8 @@
 index emulated on this GPU, with the per-phase cycle counters of the -DTPQ_DEBUG_KNOBS build.
 
 usage: TPQ_B200_LIB=torchpq_b200/libtpq_b200_dbg.so python scripts/sweep_scan.py <workload> [shard_world ...]
-       (knobs of the debug build: TPQ_SCAN_CFG=8x2|8x3|16x1|4x4, TPQ_BOOT_R=1|2, TPQ_BOOT_MODE=1 (merge tree, the product's
-        bootstrap) | 0 (one-barrier quick start), TPQ_LUT_MODE=staged, TPQ_RES_MODE=staged2|staged3)
+       (knobs of the debug build: TPQ_SCAN_CFG=8x2|8x3|16x1|4x4, TPQ_BOOT_R=1|2, TPQ_BOOT_MODE=1 (merge tree, this build's
+        default) | 0 (one-barrier quick start, the product library's bootstrap), TPQ_LUT_MODE=staged, TPQ_RES_MODE=staged2|staged3)
 Prints one JSON line per configuration and appends them to gpurun_out/sweep_scan.jsonl."""
 import ctypes, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -21,18 +21,24 @@ CELL = {"cell_lut_kernel<2>", "ivfpq_scan_kernel<64, 8, 2, 0, false>", "ivfpq_ce
         "merge_topk_kernel"}
 
 
-def launched(fn):
-    """names (namespace and parameter list stripped) of the scan, LUT, cell and merge kernels that fn() launches"""
+def launched(fn, windows=3):
+    """names (namespace and parameter list stripped) of the scan, LUT, cell and merge kernels that fn() launches.
+    Late in a long pytest process the profiler has dropped the first launch of a window, and now and then every launch
+    of one; so each window opens with a throwaway kernel, and the names seen in a few windows are pooled (fn() launches
+    the same kernels on every call)."""
     fn()                                                                  # layout, module loads
     torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
     names = set()
-    for e in prof.events():
-        n = re.sub(r"^void ", "", e.name).replace("tpq::", "").split("(")[0]
-        if any(s in n for s in ("scan", "lut", "cell_", "merge")):
-            names.add(n)
+    for _ in range(windows):
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            torch.ones(1, device="cuda").add_(1)
+            torch.cuda.synchronize()
+            fn()
+            torch.cuda.synchronize()
+        for e in prof.events():
+            n = re.sub(r"^void ", "", e.name).replace("tpq::", "").split("(")[0]
+            if any(s in n for s in ("scan", "lut", "cell_", "merge")):
+                names.add(n)
     return names
 
 

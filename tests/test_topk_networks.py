@@ -1,9 +1,13 @@
-"""CPU: an executable specification of the register bitonic networks and the merge-tree bootstrap of
-torchpq_b200/csrc/common.cuh (reg_sort / reg_merge / warp_bitonic_merge_desc / warp_merge_run / warp_merge_runs /
-CtaTopK::cta_bootstrap).  The functions below are line-by-line transliterations of the index arithmetic of those
+"""CPU: an executable specification of the register bitonic networks and the top-k selection protocol of
+torchpq_b200/csrc/common.cuh (reg_sort / reg_merge / warp_bitonic_merge_desc / warp_merge_run / warp_merge_runs, and
+CtaTopK / WarpTopK).  The functions below are line-by-line transliterations of the index arithmetic of those
 routines (element r*32 + lane of a warp's run, shuffle distance j, direction bit k, run regions 64 keys apart, the
 gap-closing copy for 32-key runs) with "all lanes at once" semantics for a shuffle stage; they are checked against
-`sorted`.  The GPU tests check the kernels' results; this file pins the networks' index math where no GPU is needed."""
+`sorted`.  The product library bootstraps the scan's threshold with CtaTopK::cta_quickstart, specified below together
+with push / flush / merge_locked / merge_run_capped / cta_drain under a seeded scheduler of warps and lock contention.
+CtaTopK::cta_bootstrap, the merge tree, is compiled only into the -DTPQ_DEBUG_KNOBS build, where it is the default; it
+is specified here too.  The GPU tests check the kernels' results; this file pins the protocol where no GPU is
+needed."""
 import random
 
 import pytest
@@ -174,3 +178,254 @@ def test_merge_tree_bootstrap(nw, R, kp):
         got = cta_bootstrap(keys, nw, R, kp)
         expect = sorted((k for w in keys for k in w), reverse=True)[:kp]
         assert got == expect + [0] * (kp - len(expect))
+
+
+# ----------------------------------------------------------------------------------------------- the shipped protocol
+# CtaTopK as the product build runs it in ivfpq_scan_kernel (scan.cu): cta_quickstart on the first R blocks of every
+# warp, then push / flush (try-lock above 32 staged keys, forced above 64) / merge_run_capped / merge_locked (with its
+# early return) while the warps take blocks from a shared cursor, then cta_drain; and WarpTopK as cell_select_kernel runs
+# it.  A seeded scheduler picks which warp takes the next block, whether the lock is busy at each try, and whether a
+# warp's copy of the threshold is stale; the networks are the transliterations above.
+K_STAGE = 96                    # CtaTopK staging entries per warp (kStage)
+
+
+def list_capacity(k):
+    p = 1
+    while p < max(k, 32):
+        p <<= 1
+    return p
+
+
+def _run(keys, R, asc=True):
+    """a warp's staged keys (missing ones 0) sorted in registers: reg_sort<R, ASC>"""
+    x = _regs(list(keys) + [0] * (32 * R - len(keys)), R)
+    reg_sort(x, R, asc)
+    return x
+
+
+class CtaSim:
+    def __init__(self, k, nw, rng, p_busy):
+        self.k, self.nw, self.kp = k, nw, list_capacity(k)
+        self.lst, self.thr = [0] * self.kp, 0
+        self.buf = [[] for _ in range(nw)]
+        self.rng, self.p_busy = rng, p_busy
+        self.paths = set()
+
+    def _merged(self):
+        assert self.lst == sorted(self.lst, reverse=True), "the shared list is sorted after every merge"
+
+    def merge_locked(self, x, R):
+        top = x[R - 1][31]
+        if top < self.thr:                                     # nothing staged can still be in the top k
+            self.paths.add("early return")
+            return
+        if top > self.lst[self.k - 1]:
+            merge_run(self.lst, self.kp, x, R)
+            self._merged()
+            self.thr = max(self.thr, self.lst[self.k - 1])
+
+    def merge_run_capped(self, x, R):
+        if R == 4 and self.kp < 128:
+            self.paths.add(f"capped R=4 kp={self.kp}")
+            if self.kp == 32:
+                self.merge_locked([x[R - 1]], 1)
+            else:
+                self.merge_locked([x[R // 2], x[R - 1]], 2)
+        elif R == 2 and self.kp == 32:
+            self.paths.add("capped R=2 kp=32")
+            self.merge_locked([x[R - 1]], 1)
+        else:
+            self.merge_locked(x, R)
+
+    def flush(self, w, force):
+        b = self.buf[w]
+        if not b:
+            return
+        if not force and self.rng.random() < self.p_busy:      # another warp holds the lock: keep scanning
+            self.paths.add("lock busy")
+            return
+        if len(b) <= 32:
+            self.merge_locked(_run(b, 1), 1)
+        elif len(b) <= 64:
+            self.merge_run_capped(_run(b, 2), 2)
+        else:
+            self.paths.add("forced 65-96")
+            self.merge_run_capped(_run(b, 4), 4)
+        b.clear()
+
+    def push(self, w, keys):
+        b = self.buf[w]
+        b.extend(keys)
+        assert len(b) <= K_STAGE, "a warp stages at most kStage keys"
+        if len(b) > 32:
+            self.flush(w, len(b) > K_STAGE - 32)
+
+    def quickstart(self, staged, R):
+        """staged[w]: the 32 R keys of warp w's bootstrap blocks (0 for missing vectors)"""
+        runs = []
+        for w in range(self.nw):
+            x = _regs(list(staged[w]) + [0] * (64 - 32 * R), 2)
+            reg_sort(x, 2)                                     # descending: ranks 0..63
+            runs.append(_flat(x, 2))
+        q = (self.k + self.nw - 1) // self.nw
+        bound = min(r[q - 1] if q <= 32 * R else 0 for r in runs)
+        if bound == 0:
+            self.paths.add("no bound")
+        self.thr = max(self.thr, bound)
+        for w, r in enumerate(runs):
+            kept = [i for i, v in enumerate(r) if v != 0 and v >= bound]
+            assert kept == list(range(len(kept))), "the kept keys are a prefix of the sorted run"
+            self.buf[w] = r[:len(kept)]
+
+    def drain(self):
+        t = self.thr
+        left = [v for b in self.buf for v in b[:K_STAGE] if v != 0 and v >= t]
+        if any(v == t for v in left):
+            self.paths.add("drain keeps the bound")
+        for c0 in range(0, len(left), 64):
+            x = _run(left[c0:c0 + 64], 2)
+            if self.kp == 32:
+                merge_run(self.lst, self.kp, [x[1]], 1)
+            else:
+                merge_run(self.lst, self.kp, x, 2)
+            self._merged()
+        self.buf = [[] for _ in range(self.nw)]
+
+
+def simulate_scan(blocks, k, nw, seed, R=2, p_busy=0.5, p_stale=0.3):
+    """ivfpq_scan_kernel's selection over `blocks` (lists of 32 keys, 0 = not live) -> (the CTA's list, paths seen)"""
+    rng = random.Random(seed)
+    cta = CtaSim(k, nw, rng, p_busy)
+    n = len(blocks)
+    staged = [[key for r in range(R) for key in (blocks[w + r * nw] if w + r * nw < n else [0] * 32)]
+              for w in range(nw)]
+    cta.quickstart(staged, R)
+    cursor, thr_seen, active = R * nw, [cta.thr] * nw, list(range(nw))
+    while active:
+        w = rng.choice(active)
+        if cursor >= n:
+            active.remove(w)
+            continue
+        b = blocks[cursor]
+        cursor += 1
+        if rng.random() >= p_stale:
+            thr_seen[w] = cta.thr                              # the running k-th best, read at most once per block
+        cta.push(w, [key for key in b if key != 0 and key > thr_seen[w]])
+    cta.drain()
+    return cta.lst, cta.paths
+
+
+def warp_select(start, cand, k):
+    """cell_select_kernel: WarpTopK seeded with a sorted list of k keys (the pass-1 list), pushed 32 candidates at a
+    time against its own k-th best, flushed above 32 staged keys and at the end"""
+    kp = list_capacity(k)
+    lst = list(start) + [0] * (kp - len(start))
+    buf = []
+
+    def flush():
+        if not buf:
+            return
+        if len(buf) <= 32:
+            merge_run(lst, kp, _run(buf, 1), 1)
+        else:
+            x = _run(buf, 2)
+            if kp == 32:
+                merge_run(lst, kp, [x[1]], 1)
+            else:
+                merge_run(lst, kp, x, 2)
+        assert lst == sorted(lst, reverse=True)
+        buf.clear()
+
+    for i0 in range(0, len(cand), 32):
+        th = lst[k - 1]
+        buf.extend(v for v in cand[i0:i0 + 32] if v > th)
+        assert len(buf) <= 64
+        if len(buf) > 32:
+            flush()
+    flush()
+    return lst
+
+
+def pattern_keys(pattern, n_blocks, k, nw, seed, R=2):
+    """keys of n_blocks blocks in visit order for one of the designed score patterns (tests/designed_state.py);
+    key = score << 20 | ~position: distinct, larger is better, 0 is empty"""
+    rng = random.Random(seed)
+    n = 32 * n_blocks
+    if pattern == "ascending":
+        s = list(range(1, n + 1))
+    elif pattern == "descending":
+        s = list(range(n, 0, -1))
+    elif pattern == "equal":
+        s = [7] * n
+    elif pattern == "needle":
+        s = rng.sample(range(1, n + 1), n)
+        s[n - 5] = n + 1
+    elif pattern == "random":
+        s = rng.sample(range(1, n + 1), n)
+    elif pattern == "plateau":
+        lead = min(k - 1, n // 4)
+        s = [1 + rng.randrange(n) for _ in range(n)]
+        for i in range(n):
+            if i % 3 == 1:
+                s[i] = n + 1
+        for i in rng.sample([i for i in range(n) if i % 3 != 1], lead):
+            s[i] = n + 2 + rng.randrange(n)
+    elif pattern == "bound":
+        s = [1 + rng.randrange(n) for _ in range(n)]
+        for r in range(1, min(k, 64 * nw) + 1):
+            w, idx = (r - 1) % nw, (r - 1) // nw
+            s[(w + nw * (idx // 32)) * 32 + idx % 32] = 2 * n - r
+    else:
+        raise ValueError(pattern)
+    keys = [(v << 20) | ((1 << 20) - 1 - i) for i, v in enumerate(s)]
+    if pattern in ("equal", "needle", "random"):                # holes: partly live blocks, the last one too
+        for i in range(0, n, 7 if pattern == "equal" else 11):
+            keys[i] = 0
+        keys[n - 2] = 0
+    return [keys[b * 32:(b + 1) * 32] for b in range(n_blocks)]
+
+
+SCAN_CASES = [(nw, k) for nw in (4, 8) for k in (1, 31, 32, 33, 64, 65, 100, 128, 300)] + [(8, 513)]
+
+
+@pytest.mark.parametrize("nw, k", SCAN_CASES)
+@pytest.mark.parametrize("pattern", ["ascending", "descending", "equal", "needle", "random", "plateau", "bound"])
+def test_shipped_scan_selection(pattern, nw, k):
+    """The exact top k of every pattern under two seeded schedules; k = 300 at 4 warps and 513 at 8 exceed the quick
+    start's limit 32 * 2 * NW, so it gives no bound there."""
+    n_blocks = 2 * nw + 24
+    blocks = pattern_keys(pattern, n_blocks, k, nw, seed=k)
+    every = sorted((v for b in blocks for v in b if v), reverse=True)[:k]
+    for seed in (1, 2):
+        lst, _ = simulate_scan(blocks, k, nw, seed=seed * 1000 + k)
+        assert lst[:k] == every + [0] * (k - len(every))
+
+
+def test_shipped_scan_reaches_every_path():
+    """The schedules above are not idle: over a handful of runs the simulation takes every branch the GPU reaches
+    only by chance -- forced 65-96-key flushes, both capped merges, the early return, no bound, and a drain that keeps
+    a key equal to the bound."""
+    seen = set()
+    for pattern, nw, k, n in (("ascending", 8, 32, 40), ("ascending", 8, 100, 40), ("ascending", 4, 1, 32),
+                              ("bound", 8, 64, 40), ("random", 4, 300, 32), ("descending", 8, 256, 40),
+                              ("ascending", 8, 33, 40), ("random", 8, 1, 400)):
+        for seed in range(3):
+            seen |= simulate_scan(pattern_keys(pattern, n, k, nw, seed), k, nw, seed=seed, p_busy=0.7, p_stale=0.9)[1]
+    for p in ("forced 65-96", "capped R=4 kp=32", "capped R=4 kp=64", "capped R=2 kp=32", "early return", "lock busy",
+              "no bound", "drain keeps the bound"):
+        assert p in seen, p
+
+
+@pytest.mark.parametrize("k", [1, 31, 32, 33, 64, 100, 128, 1024])
+def test_warp_select(k):
+    rng = random.Random(k)
+    for pattern in ("ascending", "descending", "equal", "random"):
+        pool = pattern_keys(pattern, 40, k, 8, seed=k)
+        flat = [v for b in pool for v in b if v]
+        start = sorted(flat[:k], reverse=True)
+        cand = sorted(flat[k:], reverse=(pattern == "descending")) if pattern != "random" else flat[k:]
+        if pattern == "equal":
+            rng.shuffle(cand)
+        got = warp_select(start, cand, k)
+        every = sorted(flat, reverse=True)[:k]
+        assert got[:k] == every + [0] * (k - len(every))

@@ -352,9 +352,9 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
     write_keys<NW>(A, tk.list, q, slice, tid);
     return;
   }
-  // bootstrap: the first R blocks of every warp go to the list unfiltered through one register sort per warp and a
-  // log2(NW)-level merge tree, which establishes the threshold (k-th best of the first R * NW * 32 vectors) without
-  // R * NW lock-serialised flushes.
+  // bootstrap: the first R blocks of every warp, sorted in registers per warp, give the threshold a lower bound after
+  // one barrier (cta_quickstart) without R * NW lock-serialised flushes.  The merge tree (cta_bootstrap) exists only in
+  // the debug build, where it is the default.
   const int R = A.boot_r;
   if (tid == 0) *sc.next = b_begin + R * NW;                    // the bootstrap's barriers publish it
   {
