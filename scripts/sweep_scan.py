@@ -3,7 +3,8 @@ index emulated on this GPU, with the per-phase cycle counters of the -DTPQ_DEBUG
 
 usage: TPQ_B200_LIB=torchpq_b200/libtpq_b200_dbg.so python scripts/sweep_scan.py <workload> [shard_world ...]
        (knobs of the debug build: TPQ_SCAN_CFG=8x2|8x3|16x1|4x4, TPQ_BOOT_R=1|2, TPQ_BOOT_MODE=1 (merge tree, this build's
-        default) | 0 (one-barrier quick start, the product library's bootstrap), TPQ_LUT_MODE=staged, TPQ_RES_MODE=staged2|staged3)
+        default) | 0 (one-barrier quick start, the product library's bootstrap), TPQ_LUT_MODE=staged, TPQ_RES_MODE=staged2|staged3,
+        TPQ_CELL_CFG=14x6|16x5 (shape of the cell-major kernel; scripts/cell_scan_account.py sweeps it with its cycle account))
 Prints one JSON line per configuration and appends them to gpurun_out/sweep_scan.jsonl."""
 import ctypes, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -22,7 +23,7 @@ k = wl[5]
 xs = [x.to(dev) for x in bench.gen_queries(wl[1], nq, 4, dev)]
 lib = T._lib.lib
 dbg = hasattr(lib, "tpq_debug_set_phase_buffer") or "dbg" in os.environ.get("TPQ_B200_LIB", "")
-phase = torch.zeros(8, dtype=torch.int64, device=dev)
+phase = torch.zeros(16, dtype=torch.int64, device=dev)     # [8..15]: the cell-major kernel's account (cell_scan_account.py)
 if dbg:
     f = lib.tpq_debug_set_phase_buffer
     f.restype, f.argtypes = ctypes.c_int, [ctypes.c_void_p]

@@ -20,8 +20,8 @@
 //   * RES variant: residual IVFPQ (per-cell LUT = query half + precomputed cell half).
 // Sub-quantizer sums are fp32 in four interleaved partial sums (exact for integer LUTs;
 // ~1e-7 relative otherwise -- the reference's m-ascending order lives in scan_ref.cu).
-// Experiment knobs (TPQ_SCAN_CFG, TPQ_BOOT_R, TPQ_LUT_MODE) and per-phase cycle counters exist only in the
-// -DTPQ_DEBUG_KNOBS build (make dbg -> libtpq_b200_dbg.so, used by scripts/); the product library reads no environment.
+// Experiment knobs (TPQ_SCAN_CFG, TPQ_BOOT_R, TPQ_LUT_MODE, TPQ_CELL_CFG, TPQ_CELL_ABLATE) and per-phase cycle counters
+// exist only in the -DTPQ_DEBUG_KNOBS build (make dbg -> libtpq_b200_dbg.so, used by scripts/); the product library reads no environment.
 #include <stdlib.h>
 #include <string.h>
 #include <type_traits>
@@ -217,7 +217,7 @@ struct ScanArgs {
   const int* only_cnt;            // non-null: scan only the chunk's queries qi with only_cnt[qi] > only_cap (cell-major overflow)
   int only_cap;
 #ifdef TPQ_DEBUG_KNOBS
-  unsigned long long* phase;      // [8] summed clock64 deltas: prologue, bootstrap, scan, drain; [4] = CTAs
+  unsigned long long* phase;      // [16]; [0..4] summed clock64 deltas: prologue, bootstrap, scan, drain; [4] = CTAs
   int boot_mode;                  // 1 = merge-tree bootstrap (A/B against the quick start)
 #endif
 };
@@ -442,7 +442,20 @@ static int launch_merge(const uint64_t* keys_in, int nq, int n_parts, int k, int
 constexpr int kCellSlots = 3;         // LUT ring depth (64 KB each)
 constexpr int kCellNW = 12;           // warps of a cell-scan CTA
 constexpr int kCellR = 7;             // code blocks per warp held in registers (168 registers): a chunk is up to 84 blocks = 2688 vectors
-constexpr int kCellChunk = kCellNW * kCellR;
+constexpr int kCellWin = 256;         // pairs of an item whose (query, bound) records sit in shared memory at a time
+// Dynamic shared memory of a cell-scan CTA: the ring, 256 B of barriers and slot state, the warps' survivor stages, then
+// the record window (kCellWin bounds, kCellWin queries).
+constexpr size_t cell_win_offset(int nw, int r) { return (size_t)kCellSlots * lut_bytes(64) + 256 + (size_t)nw * r * 32 * 8; }
+constexpr size_t cell_smem_bytes(int nw, int r) { return cell_win_offset(nw, r) + (size_t)kCellWin * 12; }
+
+// Shared-memory accesses of the record window, by 32-bit shared address.  The window is kept apart from the pointers the
+// compiler derives from the kernel's shared base, and the pair body keeps reading its query and bound from the slot's
+// fixed words: indexed reads of the window in the pair body made ptxas move that base from a uniform register into a
+// vector register and add it to every lookup's address (4.2 instead of 3.3 instructions per lookup, sass_census.py).
+__device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
+__device__ __forceinline__ uint64_t lds_u64(uint32_t a) { uint64_t v; asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory"); return v; }
+__device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void sts_u64(uint32_t a, uint64_t v) { asm volatile("st.shared.u64 [%0], %1;" :: "r"(a), "l"(v) : "memory"); }
 constexpr int kCellBuckets = 128;     // work classes of the largest-first item order (4 per octave)
 
 struct CellItem { int32_t cell, b_lo, b_hi, pad; };   // blocks [b_lo, b_hi) of the cell (relative to its first block)
@@ -457,6 +470,13 @@ struct CellArgs {
   const uint64_t* keys;           // [nq][k] pass-1 lists; key k-1 is the query's bound
   uint64_t* surv; int* surv_cnt;  // [n][cap] survivors, [n] their count (> cap: overflow), by chunk-local query
   int q_base, k, cap;
+#ifdef TPQ_DEBUG_KNOBS
+  unsigned long long* phase;      // the phase buffer's [8..15]: warp-cycles summed over all warps in item prologue (barrier,
+                                  // code loads, first LUT wait), mbar_wait, scoring, release + issue, reservation + copy-out;
+                                  // [13] = warps, [14] = their cycles from kernel entry to exit
+  int ablate;                     // WRONG RESULTS, to bound a gain: bit 0 = no refills (every pair of an item reuses the
+                                  // first kCellSlots LUTs), bit 1 = no survivors (thr = ~0)
+#endif
 };
 
 // thread per (query, entry): count the visited pairs of entries 1 .. P-1 per cell; slot = the pair's rank in its cell
@@ -488,12 +508,12 @@ __global__ void cell_pairs_scatter_kernel(const int64_t* __restrict__ cells, int
   pair_q[cell_off[cells[(size_t)(q_base + qi) * n_probe + t % n_probe]] + s] = qi;
 }
 
-// One CTA: cell_off = exclusive prefix of cell_cnt; work items = chunks of at most kCellChunk blocks of every cell with
+// One CTA: cell_off = exclusive prefix of cell_cnt; work items = chunks of at most `chunk` blocks of every cell with
 // pairs, ordered by work (pairs x blocks) descending in classes of 4 per octave, the chunks of one cell adjacent.
 __global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__ cell_cnt, const int32_t* __restrict__ cbs,
                                                          const int64_t* __restrict__ cell_size, int n_cells,
-                                                         int* __restrict__ cell_off, CellItem* __restrict__ items,
-                                                         int* __restrict__ n_items) {
+                                                         int chunk, int* __restrict__ cell_off,
+                                                         CellItem* __restrict__ items, int* __restrict__ n_items) {
   __shared__ int hist[kCellBuckets], base[kCellBuckets], warp_sum[32], carry;
   const int tid = threadIdx.x;
   for (int i = tid; i < kCellBuckets; i += 1024) hist[i] = 0;
@@ -503,7 +523,7 @@ __global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__
     nb = cell_blocks(cbs[c], cbs[c + 1], cell_size[c]);
     const int np = cell_cnt[c];
     if (np == 0 || nb == 0) { nb = 0; return 0; }
-    const int nch = (nb + kCellChunk - 1) / kCellChunk;
+    const int nch = (nb + chunk - 1) / chunk;
     const uint32_t w = (uint32_t)np * (uint32_t)((nb + nch - 1) / nch);
     const int lg = 31 - __clz(w);
     const int sub = lg >= 2 ? (int)((w >> (lg - 2)) & 3u) : (int)((w << (2 - lg)) & 3u);
@@ -557,17 +577,42 @@ ivfpq_cell_scan_kernel(CellArgs A) {
   int* item_sh = rel + kCellSlots;                             // [2]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   uint64_t* stage = reinterpret_cast<uint64_t*>(smem + kCellSlots * lut_bytes(64) + 256) + (size_t)warp * R * 32;
+  uint32_t win_thr = smem_u32(smem + cell_win_offset(NW, R));
+  asm volatile("" : "+r"(win_thr));                            // from here on just a number to the compiler (see lds_u32)
+  const uint32_t win_q = win_thr + kCellWin * 8;
+  static_assert(kCellWin <= NW * 32, "one thread per record of the window");
   if (tid == 0) {
     for (int s = 0; s < kCellSlots; ++s) { mbar_init(&full[s], 1); rel[s] = 0; }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+#ifdef TPQ_DEBUG_KNOBS
+  // per-warp cycle account, kept in shared memory behind the stages (the kernel has no registers to spare)
+  unsigned long long* acct = reinterpret_cast<unsigned long long*>(smem + cell_smem_bytes(NW, R)) + warp * 8;
+  const bool no_refill = A.ablate & 1, no_surv = A.ablate & 2;
+  const uint32_t t_in = (uint32_t)clock();
+  uint32_t t_ph = t_in;
+  if (A.phase && lane < 8) acct[lane] = 0;
+  __syncwarp();
+  auto cell_mark = [&](int ph) {
+    if (A.phase) { const uint32_t t = (uint32_t)clock(); if (lane == 0) acct[ph] += t - t_ph; t_ph = t; }
+  };
+#define TPQ_CELL_PHASE(ph) cell_mark(ph)
+#else
+  constexpr bool no_refill = false, no_surv = false;
+#define TPQ_CELL_PHASE(ph) ((void)0)
+#endif
   uint32_t off[8];
   lane_slot_offsets(off, lane);
-  // one thread: LUT of pair i of the current cell into slot s (every warp has released the slot)
-  auto issue = [&](const int32_t* pq, int i, int s) {
-    const int qi = pq[i];
+  // one thread: LUT of pair i of the window into slot s (every warp has released the slot), its query and bound into
+  // the slot's words.
+  // It reads shared memory only: the thread that refills a slot is the last to leave it, and every warp waits for
+  // what it waits for here.
+  // It reads shared memory only: the thread that refills a slot is the last to leave it, and every warp waits for
+  // what it waits for here.
+  auto issue = [&](int i, int s) {
+    const int qi = (int)lds_u32(win_q + 4 * i);
     slot_q[s] = qi;
-    slot_thr[s] = A.keys[(size_t)(A.q_base + qi) * A.k + A.k - 1];
+    slot_thr[s] = lds_u64(win_thr + 8 * i);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the warps' reads of the slot precede the TMA write
     mbar_expect_tx(&full[s], lut_bytes(64));
     bulk_load(ring + s * lut_bytes(64), A.lut_scan + (size_t)qi * kLutGroup, lut_bytes(64), &full[s]);
@@ -584,8 +629,6 @@ ivfpq_cell_scan_kernel(CellArgs A) {
     const int32_t* pq = A.pair_q + A.cell_off[ci.cell];
     // Pair i of every item uses slot i % kCellSlots: the ring is drained at the barrier above, so it can restart at
     // slot 0, and each pair body below is compiled for its slot (the slot's offset is an LDS immediate).
-    if (tid == 0)
-      for (int i = 0; i < min(np, kCellSlots); ++i) issue(pq, i, i);
     const int b0 = A.cell_block_start[ci.cell];
     const uint32_t a0 = (uint32_t)A.cell_start[ci.cell];
     // blocks of this warp (may be <= 0); broadcast from lane 0 so that the compiler knows it is warp-uniform and the
@@ -600,12 +643,15 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         vmask[r] = __ldg(A.valid + B);
       }
     }
-    auto pair = [&](auto slot, int i) {
+    auto pair = [&](auto slot, int i, int np) {                // pair i of the window's np, in ring slot `slot`
       constexpr int s = decltype(slot)::value;
-      mbar_wait(&full[s], (parity >> s) & 1u);
-      parity ^= 1u << s;
+      if (!no_refill || i < kCellSlots) {                      // no refills: the slot was armed once, at the item's start
+        mbar_wait(&full[s], (parity >> s) & 1u);
+        parity ^= 1u << s;
+      }
+      TPQ_CELL_PHASE(i == 0 ? 0 : 1);
       const int qi = slot_q[s];
-      const uint64_t thr = slot_thr[s];
+      const uint64_t thr = no_surv ? ~0ull : slot_thr[s];
       const uint8_t* lut = ring + s * lut_bytes(64);
       int n = 0;
       #pragma unroll
@@ -622,14 +668,16 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         }
       }
       __syncwarp();
+      TPQ_CELL_PHASE(2);
       if (lane == 0) {                                         // release the slot; the last warp refills it
         int old;
         asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(smem_u32(&rel[s])) : "memory");
         if (old == NW - 1) {
           rel[s] = 0;
-          if (i + kCellSlots < np) issue(pq, i + kCellSlots, s);
+          if (!no_refill && i + kCellSlots < np) issue(i + kCellSlots, s);
         }
       }
+      TPQ_CELL_PHASE(3);
       if (n) {
         int base = 0;
         if (lane == 0) base = atomicAdd(A.surv_cnt + qi, n);
@@ -640,14 +688,37 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         }
         __syncwarp();
       }
+      TPQ_CELL_PHASE(4);
     };
     static_assert(kCellSlots == 3, "one pair body per ring slot");
-    for (int i = 0; i < np; i += kCellSlots) {
-      pair(std::integral_constant<int, 0>(), i);
-      if (i + 1 < np) pair(std::integral_constant<int, 1>(), i + 1);
-      if (i + 2 < np) pair(std::integral_constant<int, 2>(), i + 2);
+    for (int p0 = 0; p0 < np; p0 += kCellWin) {
+      // the window's records: each pair's query and its bound, key k-1 of the query's pass-1 list
+      const int nwin = min(np - p0, kCellWin);
+      if (p0) __syncthreads();                                 // every warp is done with the previous window and the ring
+      if (tid < nwin) {
+        const int qi = pq[p0 + tid];
+        sts_u32(win_q + 4 * tid, (uint32_t)qi);
+        sts_u64(win_thr + 8 * tid, A.keys[(size_t)(A.q_base + qi) * A.k + A.k - 1]);
+      }
+      __syncthreads();
+      if (tid == 0)
+        for (int i = 0; i < min(nwin, kCellSlots); ++i) issue(i, i);
+      for (int i = 0; i < nwin; i += kCellSlots) {
+        pair(std::integral_constant<int, 0>(), i, nwin);
+        if (i + 1 < nwin) pair(std::integral_constant<int, 1>(), i + 1, nwin);
+        if (i + 2 < nwin) pair(std::integral_constant<int, 2>(), i + 2, nwin);
+      }
     }
   }
+#ifdef TPQ_DEBUG_KNOBS
+  cell_mark(0);                                                // the wait at the last barrier
+  if (A.phase && lane == 0) {
+    for (int ph = 0; ph < 5; ++ph) atomicAdd(A.phase + ph, acct[ph]);
+    atomicAdd(A.phase + 5, 1ull);
+    atomicAdd(A.phase + 6, (unsigned long long)((uint32_t)clock() - t_in));
+  }
+#endif
+#undef TPQ_CELL_PHASE
 }
 
 // CTA per query: its LUT in scan layout into global memory, as the query-major kernel builds it in shared memory
@@ -697,7 +768,7 @@ static cudaEvent_t g_prof_start[kProfMax], g_prof_stop[kProfMax];
 static bool g_prof_created = false;
 
 #ifdef TPQ_DEBUG_KNOBS
-static unsigned long long* g_phase = nullptr;     // device buffer set by tpq_debug_set_phase_buffer (debug build only)
+static unsigned long long* g_phase = nullptr;     // device buffer of 16 counters, set by tpq_debug_set_phase_buffer
 #endif
 
 constexpr int kCellMinLive = 1536;    // live vectors per cell, on average, from which the cell-major scan pays
@@ -720,8 +791,10 @@ struct ScanPlan {
   bool residual, part1_in_smem;   // residual IVFPQ; its query half of the LUT in a second shared-memory table
   int MP, NW, MINB;               // the query-major kernel: ivfpq_scan_kernel<MP, NW, MINB, qm_dsub(), residual>
   int boot_r;                     // blocks per warp in the kernel's bootstrap
+  int cell_nw, cell_r;            // the cell-major kernel: ivfpq_cell_scan_kernel<cell_nw, cell_r>
 #ifdef TPQ_DEBUG_KNOBS
   int boot_mode; unsigned long long* phase;
+  int cell_ablate;
 #endif
   ScanSmem L;                     // the query-major kernel's shared memory
   SearchWs ws;
@@ -741,7 +814,7 @@ static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, const
   w.lut = off;        off += P.qm_dsub() ? 0 : align_up((size_t)P.chunk * lut_bytes(ix->m_pad), 256);
   w.keys = off;       off += align_up((size_t)nq * P.S * k * 8, 256);
   const size_t C = cm ? (size_t)ix->n_cells : 0, pairs = cm ? (size_t)P.chunk * n_probe : 0;
-  const size_t n_items = cm ? C + (size_t)ix->n_blocks / kCellChunk + 1 : 0;
+  const size_t n_items = cm ? C + (size_t)ix->n_blocks / (P.cell_nw * P.cell_r) + 1 : 0;
   w.cell_cnt = off;   off += align_up((C + 2) * 4, 256);                  // pairs per cell, then the item count and cursor
   w.cell_off = off;   off += align_up(C * 4, 256);
   w.slot = off;       off += align_up(pairs * 4, 256);
@@ -764,6 +837,7 @@ static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool 
   P.residual = ix->residual != 0;
   P.MP = ix->m_pad;
   P.boot_r = 2;
+  P.cell_nw = kCellNW; P.cell_r = kCellR;
   // LUT source: built inside the scan CTA when d/M is 1, 2, 4 or 8 (the codebook slice a CTA reads from L2, M*dsub KB,
   // is then small next to the codes it goes on to stream: C4, d/M = 8, reads 0.98 MB of codebook per 7.5 MB of codes
   // and saves the 2 x 128 KB LUT round trip through HBM plus one launch); staged through HBM by lut_kernel
@@ -804,6 +878,11 @@ static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool 
   const char* bm = getenv("TPQ_BOOT_MODE");
   P.boot_mode = bm ? atoi(bm) : 1;
   P.phase = g_phase;
+  const char* cc = getenv("TPQ_CELL_CFG");            // "<warps>x<blocks per warp>" of the cell-major kernel
+  if (cc && !strcmp(cc, "14x6")) { P.cell_nw = 14; P.cell_r = 6; }
+  if (cc && !strcmp(cc, "16x5")) { P.cell_nw = 16; P.cell_r = 5; }
+  const char* ca = getenv("TPQ_CELL_ABLATE");         // bit 0: no refills, bit 1: no survivors (CellArgs::ablate)
+  P.cell_ablate = ca ? atoi(ca) & 3 : 0;
 #endif
   // Cell-major scan when a pair's LUT (64 KB) is clearly smaller than the codes of the cell it meets: the plain index at
   // M <= 64, with an in-kernel LUT build, whose cells hold more than kCellMinLive live vectors (codes) on average, on an
@@ -931,7 +1010,12 @@ static int cell_stage(const ScanPlan& P, const ScanJob& J, ScanKernel qmajor, Sc
   int* surv_cnt = reinterpret_cast<int*>(w + W.surv_cnt);
 
   auto cscan = ivfpq_cell_scan_kernel<kCellNW, kCellR>;
-  const size_t cs_smem = (size_t)kCellSlots * lut_bytes(64) + 256 + (size_t)kCellChunk * 32 * 8;
+  size_t cs_smem = cell_smem_bytes(P.cell_nw, P.cell_r);
+#ifdef TPQ_DEBUG_KNOBS
+  if (P.cell_nw == 14) cscan = ivfpq_cell_scan_kernel<14, 6>;
+  if (P.cell_nw == 16) cscan = ivfpq_cell_scan_kernel<16, 5>;
+  cs_smem += (size_t)P.cell_nw * 64;                                      // the warps' cycle accounts
+#endif
   TPQ_CUDA(cudaFuncSetAttribute(cscan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs_smem));
   const size_t sel_smem = (size_t)4 * (kp + kTopkBuf) * 8;
   TPQ_CUDA(cudaFuncSetAttribute(cell_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sel_smem));
@@ -947,7 +1031,8 @@ static int cell_stage(const ScanPlan& P, const ScanJob& J, ScanKernel qmajor, Sc
   A.n_probe_list = ones;
   qmajor<<<n, P.NW * 32, P.L.total, st>>>(A, P.L);                        // pass 1: entry 0 of every query
   TPQ_LAUNCH_CHECK("ivfpq_scan_kernel");
-  cell_plan_kernel<<<1, 1024, 0, st>>>(cell_cnt, ix->cell_block_start, ix->cell_size, C, cell_off, items, n_items);
+  cell_plan_kernel<<<1, 1024, 0, st>>>(cell_cnt, ix->cell_block_start, ix->cell_size, C, P.cell_nw * P.cell_r, cell_off,
+                                       items, n_items);
   TPQ_LAUNCH_CHECK("cell_plan_kernel");
   cell_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(J.cells, q0, n, J.n_probe, slot, cell_off, pair_q);
   TPQ_LAUNCH_CHECK("cell_pairs_scatter_kernel");
@@ -956,7 +1041,10 @@ static int cell_stage(const ScanPlan& P, const ScanJob& J, ScanKernel qmajor, Sc
   CA.cell_start = ix->cell_start; CA.lut_scan = lut_ws; CA.cell_off = cell_off; CA.cell_cnt = cell_cnt; CA.pair_q = pair_q;
   CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
   CA.q_base = q0; CA.k = J.k; CA.cap = cap;
-  cscan<<<device_sm_count(), kCellNW * 32, cs_smem, st>>>(CA);
+#ifdef TPQ_DEBUG_KNOBS
+  CA.phase = P.phase ? P.phase + 8 : nullptr; CA.ablate = P.cell_ablate;
+#endif
+  cscan<<<device_sm_count(), P.cell_nw * 32, cs_smem, st>>>(CA);
   TPQ_LAUNCH_CHECK("ivfpq_cell_scan_kernel");
   cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(keys, surv, surv_cnt, q0, n, J.k, kp, cap);
   TPQ_LAUNCH_CHECK("cell_select_kernel");
@@ -1065,7 +1153,7 @@ static int search(const tpq_index* ix, Probes p, int nq, int n_probe, int k, int
 using namespace tpq;
 
 #ifdef TPQ_DEBUG_KNOBS
-extern "C" int tpq_debug_set_phase_buffer(unsigned long long* dev_buf8) { g_phase = dev_buf8; return TPQ_OK; }
+extern "C" int tpq_debug_set_phase_buffer(unsigned long long* dev_buf16) { g_phase = dev_buf16; return TPQ_OK; }
 #endif
 
 extern "C" int tpq_profile_enable(int on) {
