@@ -1,7 +1,7 @@
 """GPU: the scans' top-k selection on designed, rank-adversarial scores (tests/designed_state.py).
 
 Random codes settle the running k-th best within a few blocks, after which almost nothing beats the threshold, so the
-rare paths of the selection protocol (common.cuh: CtaTopK's try-lock and forced flushes, merge_run_capped, the quick
+rare paths of the selection protocol (common.cuh: CtaTopK's try-lock and forced flushes, merge_capped, the quick
 start's bound and the drain that keeps keys equal to it; scan.cu: the cell-major survivor reservation at exactly its
 capacity, multi-item cells, the 16 384-query chunk; merge_topk_kernel over empty slices and shards) are reached seldom
 or never.  Here every slot's score is an exact integer laid out along the scan's visit order -- ascending, descending,

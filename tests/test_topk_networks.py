@@ -4,7 +4,8 @@ CtaTopK / WarpTopK).  The functions below are line-by-line transliterations of t
 routines (element r*32 + lane of a warp's run, shuffle distance j, direction bit k, run regions 64 keys apart, the
 gap-closing copy for 32-key runs) with "all lanes at once" semantics for a shuffle stage; they are checked against
 `sorted`.  The product library bootstraps the scan's threshold with CtaTopK::cta_quickstart, specified below together
-with push / flush / merge_locked / merge_run_capped / cta_drain under a seeded scheduler of warps and lock contention.
+with push / flush / merge_staged / merge_capped / merge_locked / cta_drain under a seeded scheduler of warps and lock
+contention.
 CtaTopK::cta_bootstrap, the merge tree, is compiled only into the -DTPQ_DEBUG_KNOBS build, where it is the default; it
 is specified here too.  The GPU tests check the kernels' results; this file pins the protocol where no GPU is
 needed."""
@@ -158,7 +159,7 @@ def test_register_sort_and_merge(R, asc):
 @pytest.mark.parametrize("R", [1, 2, 4])
 def test_merge_run_into_list(kp, R):
     if 32 * R > kp:
-        pytest.skip("the run is capped to the list length before the merge (merge_run_capped)")
+        pytest.skip("the run is capped to the list length before the merge (merge_capped)")
     rng = random.Random(kp + R)
     for _ in range(8):
         lst = sorted([rng.randrange(0, 1000) for _ in range(kp)], reverse=True)
@@ -182,7 +183,7 @@ def test_merge_tree_bootstrap(nw, R, kp):
 
 # ----------------------------------------------------------------------------------------------- the shipped protocol
 # CtaTopK as the product build runs it in ivfpq_scan_kernel (scan.cu): cta_quickstart on the first R blocks of every
-# warp, then push / flush (try-lock above 32 staged keys, forced above 64) / merge_run_capped / merge_locked (with its
+# warp, then push / flush (try-lock above 32 staged keys, forced above 64) / merge_staged / merge_capped / merge_locked (with its
 # early return) while the warps take blocks from a shared cursor, then cta_drain; and WarpTopK as cell_select_kernel runs
 # it.  A seeded scheduler picks which warp takes the next block, whether the lock is busy at each try, and whether a
 # warp's copy of the threshold is stale; the networks are the transliterations above.
@@ -197,7 +198,7 @@ def list_capacity(k):
 
 
 def _run(keys, R, asc=True):
-    """a warp's staged keys (missing ones 0) sorted in registers: reg_sort<R, ASC>"""
+    """a warp's staged keys (missing ones 0) sorted in registers: load_sorted_run<R>, reg_sort<R, ASC>"""
     x = _regs(list(keys) + [0] * (32 * R - len(keys)), R)
     reg_sort(x, R, asc)
     return x
@@ -224,16 +225,14 @@ class CtaSim:
             self._merged()
             self.thr = max(self.thr, self.lst[self.k - 1])
 
-    def merge_run_capped(self, x, R):
-        if R == 4 and self.kp < 128:
-            self.paths.add(f"capped R=4 kp={self.kp}")
-            if self.kp == 32:
-                self.merge_locked([x[R - 1]], 1)
-            else:
-                self.merge_locked([x[R // 2], x[R - 1]], 2)
-        elif R == 2 and self.kp == 32:
-            self.paths.add("capped R=2 kp=32")
+    def merge_capped(self, x, R):
+        """merge_capped with merge = merge_locked: only the run's kp largest, its last registers, can matter"""
+        if R > 1 and self.kp == 32:
+            self.paths.add(f"capped R={R} kp=32")
             self.merge_locked([x[R - 1]], 1)
+        elif R > 2 and self.kp == 64:
+            self.paths.add(f"capped R={R} kp=64")
+            self.merge_locked([x[R - 2], x[R - 1]], 2)
         else:
             self.merge_locked(x, R)
 
@@ -244,13 +243,13 @@ class CtaSim:
         if not force and self.rng.random() < self.p_busy:      # another warp holds the lock: keep scanning
             self.paths.add("lock busy")
             return
-        if len(b) <= 32:
+        if len(b) <= 32:                                       # merge_staged<4>
             self.merge_locked(_run(b, 1), 1)
         elif len(b) <= 64:
-            self.merge_run_capped(_run(b, 2), 2)
+            self.merge_capped(_run(b, 2), 2)
         else:
             self.paths.add("forced 65-96")
-            self.merge_run_capped(_run(b, 4), 4)
+            self.merge_capped(_run(b, 4), 4)
         b.clear()
 
     def push(self, w, keys):
@@ -282,12 +281,14 @@ class CtaSim:
         left = [v for b in self.buf for v in b[:K_STAGE] if v != 0 and v >= t]
         if any(v == t for v in left):
             self.paths.add("drain keeps the bound")
-        for c0 in range(0, len(left), 64):
-            x = _run(left[c0:c0 + 64], 2)
-            if self.kp == 32:
-                merge_run(self.lst, self.kp, [x[1]], 1)
+        for c0 in range(0, len(left), 64):                     # merge_staged<2> with merge = warp_merge_run
+            chunk = left[c0:c0 + 64]
+            if len(chunk) <= 32:
+                merge_run(self.lst, self.kp, _run(chunk, 1), 1)
+            elif self.kp == 32:
+                merge_run(self.lst, self.kp, [_run(chunk, 2)[1]], 1)
             else:
-                merge_run(self.lst, self.kp, x, 2)
+                merge_run(self.lst, self.kp, _run(chunk, 2), 2)
             self._merged()
         self.buf = [[] for _ in range(self.nw)]
 
@@ -317,7 +318,8 @@ def simulate_scan(blocks, k, nw, seed, R=2, p_busy=0.5, p_stale=0.3):
 
 def warp_select(start, cand, k):
     """cell_select_kernel: WarpTopK seeded with a sorted list of k keys (the pass-1 list), pushed 32 candidates at a
-    time against its own k-th best, flushed above 32 staged keys and at the end"""
+    time against its own k-th best, flushed above 32 staged keys and at the end (flush: merge_staged<2> with merge =
+    warp_merge_run)"""
     kp = list_capacity(k)
     lst = list(start) + [0] * (kp - len(start))
     buf = []

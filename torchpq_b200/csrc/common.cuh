@@ -54,22 +54,23 @@ __device__ __forceinline__ float    key_score(uint64_t k) { return ord_to_score(
 __device__ __forceinline__ uint32_t key_addr(uint64_t k)  { return 0xFFFFFFFFu - (uint32_t)k; }
 
 #ifdef __CUDACC__
+// Inclusive prefix sum over the lanes of a full warp: returns the sum of v over lanes 0 .. lane.
+template <class T>
+__device__ __forceinline__ T warp_inclusive_scan(T v, int lane) {
+  #pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+  return v;
+}
+
 // One 1024-value tile of a CTA-wide inclusive prefix sum (blockDim.x == 1024, called by every thread): returns carry +
 // the sum of v over threads 0 .. threadIdx.x, and advances carry (shared memory) by the tile's total.  wsum: [32] shared.
 template <class T>
 __device__ __forceinline__ T cta_inclusive_scan(T v, T* wsum, T& carry) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  T incl = v;
-  #pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+  const T incl = warp_inclusive_scan(v, lane);
   if (lane == 31) wsum[warp] = incl;
   __syncthreads();
-  if (warp == 0) {
-    T w = wsum[lane];
-    #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += t; }
-    wsum[lane] = w;                                                   // inclusive over warps
-  }
+  if (warp == 0) wsum[lane] = warp_inclusive_scan(wsum[lane], lane);   // inclusive over warps
   __syncthreads();
   const T r = carry + (warp ? wsum[warp - 1] : T(0)) + incl;
   __syncthreads();
@@ -221,7 +222,46 @@ __device__ __forceinline__ void warp_merge_runs(uint64_t* A, uint64_t* B, int le
   if (!top_only) warp_bitonic_merge_desc(B, len, lane);
 }
 
-constexpr int kTopkBuf = 64;      // staging-buffer entries per warp
+// ----------------------------------------------------------------------------- staged candidates
+// A selector stages the keys that pass its filter in an unsorted buffer, and from time to time sorts the staged run in
+// registers and merges it into its sorted list.  The three steps below are the only copies of their rules.
+
+// The lanes with `pass` append their keys to buf[cnt ..) in lane order; returns how many were appended (warp-uniform).
+__device__ __forceinline__ int warp_append(uint64_t* buf, int cnt, bool pass, uint64_t key, int lane) {
+  const unsigned m = __ballot_sync(0xffffffffu, pass);
+  if (pass) buf[cnt + __popc(m & ((1u << lane) - 1))] = key;
+  return __popc(m);
+}
+
+constexpr int kTopkBuf = 64;      // WarpTopK staging entries per warp
+constexpr int kStage = 96;        // CtaTopK staging entries per warp: flush is attempted above 32, forced above 64
+
+// x <- the n <= 32*R keys staged at buf, padded with empty keys, sorted ASCENDING (x[r] = element r*32 + lane).  No
+// buffer stages more than kStage keys, so a register past that is empty without a look at n.
+template <int R>
+__device__ __forceinline__ void load_sorted_run(uint64_t (&x)[R], const uint64_t* buf, int n, int lane) {
+  #pragma unroll
+  for (int r = 0; r < R; ++r) x[r] = (r * 32 < kStage && r * 32 + lane < n) ? buf[r * 32 + lane] : 0ull;
+  reg_sort<R, true>(x, lane);
+}
+
+// The cap: of an ascending run of 32*R keys only the kp largest can enter a list of kp slots, and they are its last
+// registers.  merge(y) receives the run, or its last kp keys when it is longer than the list.
+template <int R, class Merge>
+__device__ __forceinline__ void merge_capped(const uint64_t (&x)[R], int kp, Merge merge) {
+  if (R > 1 && kp == 32) { const uint64_t y[1] = {x[R - 1]}; merge(y); }
+  else if (R > 2 && kp == 64) { const uint64_t y[2] = {x[R - 2], x[R - 1]}; merge(y); }
+  else merge(x);
+}
+
+// Sort the n staged keys of buf (0 < n <= 32*RMAX) into the shortest run that holds them and hand it, capped to kp, to
+// merge: warp_merge_run into a list the warp owns, CtaTopK::merge_locked into the CTA's.
+template <int RMAX, class Merge>
+__device__ __forceinline__ void merge_staged(const uint64_t* buf, int n, int kp, int lane, Merge merge) {
+  if (n <= 32) { uint64_t x[1]; load_sorted_run(x, buf, n, lane); merge(x); }
+  else if (RMAX == 2 || n <= 64) { uint64_t x[2]; load_sorted_run(x, buf, n, lane); merge_capped(x, kp, merge); }
+  else { uint64_t x[4]; load_sorted_run(x, buf, n, lane); merge_capped(x, kp, merge); }
+}
 
 // Per-warp top-k selector: sorted list of KP keys + an unsorted staging buffer.
 // Candidates are appended with push(); when the buffer cannot take another full
@@ -243,24 +283,14 @@ struct WarpTopK {
 
   __device__ __forceinline__ void flush(int lane) {
     if (cnt == 0) return;
-    if (cnt <= 32) {
-      uint64_t x[1] = {lane < cnt ? buf[lane] : 0ull};
-      reg_sort<1, true>(x, lane);
-      warp_merge_run<1>(list, kp, x, lane);
-    } else {
-      uint64_t x[2] = {buf[lane], lane + 32 < cnt ? buf[lane + 32] : 0ull};
-      reg_sort<2, true>(x, lane);
-      if (kp == 32) { uint64_t y[1] = {x[1]}; warp_merge_run<1>(list, kp, y, lane); }   // the 32 largest of the run
-      else warp_merge_run<2>(list, kp, x, lane);
-    }
+    merge_staged<2>(buf, cnt, kp, lane, [&](const auto& x) { warp_merge_run(list, kp, x, lane); });
     cnt = 0;
   }
   // pass: this lane has a candidate.  Returns true if a flush happened (threshold may have risen).
   __device__ __forceinline__ bool push(bool pass, uint64_t key, int lane) {
-    unsigned m = __ballot_sync(0xffffffffu, pass);
-    if (m == 0) return false;
-    if (pass) buf[cnt + __popc(m & ((1u << lane) - 1))] = key;
-    cnt += __popc(m);
+    const int n = warp_append(buf, cnt, pass, key, lane);
+    if (n == 0) return false;
+    cnt += n;
     __syncwarp();
     if (cnt > kTopkBuf - 32) { flush(lane); return true; }
     return false;
@@ -273,7 +303,8 @@ struct WarpTopK {
 // CTA lock and merges it into the shared list; the other warps keep scanning against the
 // (slightly stale, always valid) threshold in *thr.  Exact: a candidate is only ever dropped
 // when k better ones are already in the list.
-constexpr int kStage = 96;        // CtaTopK staging entries per warp: flush is attempted above 32, forced above 64
+// The selector owns its shared memory: a kernel reserves bytes(nw, kp) at an 8-byte aligned offset and hands the
+// address to init(), which lays out  thr | lock, drain counter | rep[nw] | list[kp] | nw staging buffers of kStage keys.
 struct CtaTopK {
   uint64_t* list;               // [kp] descending, shared by the CTA
   unsigned long long* thr;      // k-th best of `list` (0 while fewer than k merged)
@@ -281,10 +312,18 @@ struct CtaTopK {
   uint64_t* buf;                // [kStage] this warp's staging buffer
   int kp, k, cnt;
 
-  // call from every thread of the CTA, then __syncthreads()
-  __device__ __forceinline__ void init(uint64_t* list_, unsigned long long* thr_, int* lock_, uint64_t* buf_,
-                                       int kp_, int k_) {
-    list = list_; thr = thr_; lock = lock_; buf = buf_; kp = kp_; k = k_; cnt = 0;
+  static constexpr size_t bytes(int nw, int kp) { return 8 * (2 + (size_t)nw + (size_t)kp + (size_t)nw * kStage); }
+  // the quick start's report of each warp; the staging buffers of all warps, scratch once their keys are in registers
+  __device__ __forceinline__ uint64_t* rep() const { return reinterpret_cast<uint64_t*>(thr) + 2; }
+  __device__ __forceinline__ uint64_t* scratch() const { return list + kp; }
+
+  // call from every thread of the CTA (nw warps), then __syncthreads()
+  __device__ __forceinline__ void init(void* smem, int nw, int warp, int kp_, int k_) {
+    thr = reinterpret_cast<unsigned long long*>(smem);
+    lock = reinterpret_cast<int*>(thr + 1);
+    list = rep() + nw;
+    kp = kp_; k = k_; cnt = 0;
+    buf = scratch() + (size_t)warp * kStage;
     for (int i = threadIdx.x; i < kp; i += blockDim.x) list[i] = 0;
     if (threadIdx.x == 0) { *thr = 0ull; lock[0] = 0; lock[1] = 0; }
   }
@@ -317,18 +356,6 @@ struct CtaTopK {
     __syncwarp();
     if (lane == 0) atomicExch(lock, 0);
   }
-  // the run x (ascending, 32*R keys) may be longer than the list: only its kp largest can matter
-  template <int R>
-  __device__ __forceinline__ void merge_run_capped(const uint64_t (&x)[R], int lane) {
-    if (R == 4 && kp < 128) {
-      if (kp == 32) { uint64_t y[1] = {x[R - 1]}; merge_locked<1>(y, lane); }
-      else { uint64_t y[2] = {x[R / 2], x[R - 1]}; merge_locked<2>(y, lane); }
-    } else if (R == 2 && kp == 32) {
-      uint64_t y[1] = {x[R - 1]}; merge_locked<1>(y, lane);
-    } else {
-      merge_locked<R>(x, lane);
-    }
-  }
   // force == false: if another warp holds the lock, do nothing -- the caller keeps scanning and retries at its next
   // push (a warp that waits for the lock does no work AND its spinning slows the holder down).
   __device__ __forceinline__ void flush(int lane, bool force) {
@@ -338,27 +365,14 @@ struct CtaTopK {
       if (lane == 0) busy = *reinterpret_cast<volatile int*>(lock);
       if (__shfl_sync(0xffffffffu, busy, 0)) return;
     }
-    if (cnt <= 32) {
-      uint64_t x[1] = {lane < cnt ? buf[lane] : 0ull};
-      reg_sort<1, true>(x, lane);
-      merge_locked<1>(x, lane);
-    } else if (cnt <= 64) {
-      uint64_t x[2] = {buf[lane], lane + 32 < cnt ? buf[lane + 32] : 0ull};
-      reg_sort<2, true>(x, lane);
-      merge_run_capped<2>(x, lane);
-    } else {
-      uint64_t x[4] = {buf[lane], buf[lane + 32], lane + 64 < cnt ? buf[lane + 64] : 0ull, 0ull};
-      reg_sort<4, true>(x, lane);
-      merge_run_capped<4>(x, lane);
-    }
+    merge_staged<4>(buf, cnt, kp, lane, [&](const auto& x) { merge_locked(x, lane); });
     __syncwarp();
     cnt = 0;
   }
   __device__ __forceinline__ void push(bool pass, uint64_t key, int lane) {
-    unsigned m = __ballot_sync(0xffffffffu, pass);
-    if (m == 0) return;
-    if (pass) buf[cnt + __popc(m & ((1u << lane) - 1))] = key;
-    cnt += __popc(m);
+    const int n = warp_append(buf, cnt, pass, key, lane);
+    if (n == 0) return;
+    cnt += n;
     __syncwarp();
     if (cnt > 32) flush(lane, cnt > kStage - 32);
   }
@@ -368,7 +382,7 @@ struct CtaTopK {
   // >= it), published after ONE barrier -- no cross-warp merge at all (the merge tree of cta_bootstrap costs log2(nw)
   // + 3 barriers).  Each warp keeps the keys >= the bound staged; they reach the list
   // through the ordinary flushes.  k > 32 * R * nw: no bound can be given, everything stays staged.
-  __device__ __forceinline__ void cta_quickstart(uint64_t* rep, int nw, int R, int lane, int warp) {
+  __device__ __forceinline__ void cta_quickstart(int nw, int R, int lane, int warp) {
     uint64_t x[2] = {buf[lane], R == 2 ? buf[lane + 32] : 0ull};
     reg_sort<2>(x, lane);                                            // descending: x[0] = ranks 0..31, x[1] = ranks 32..63
     const int q = (k + nw - 1) / nw;
@@ -378,9 +392,9 @@ struct CtaTopK {
       const uint64_t b = (uint64_t)__shfl_sync(0xffffffffu, (unsigned long long)x[1], (q - 1) & 31);
       mine = q <= 32 ? a : b;
     }
-    if (lane == 0) rep[warp] = mine;                                 // rep: nw keys of shared memory, written once per CTA
+    if (lane == 0) rep()[warp] = mine;                               // written once per CTA
     __syncthreads();
-    uint64_t bound = rep[lane < nw ? lane : 0];
+    uint64_t bound = rep()[lane < nw ? lane : 0];
     #pragma unroll 1
     for (int o = 16; o > 0; o >>= 1) bound = key_min(bound, shfl_xor64(bound, o));
     if (threadIdx.x == 0) atomicMax(thr, (unsigned long long)bound);
@@ -396,8 +410,9 @@ struct CtaTopK {
   // missing vectors): each warp sorts its run in registers, the runs are merged pairwise in a log2(nw)-level tree
   // (runs are capped at kp keys), and warp 0 merges the survivor into the list and publishes the threshold --
   // log2(nw) + 3 barriers instead of a CTA-wide bitonic sort (45 barriers for 512 keys) or nw lock-serialised flushes.
-  // `scratch` = the staging area of all warps (nw * kStage keys), used as nw runs 64 keys apart; nw a power of two.
-  __device__ __forceinline__ void cta_bootstrap(uint64_t* scratch, int nw, int R, int lane, int warp) {
+  // The staging area of all warps (nw * kStage keys) is used as nw runs 64 keys apart; nw a power of two.
+  __device__ __forceinline__ void cta_bootstrap(int nw, int R, int lane, int warp) {
+    uint64_t* scratch = this->scratch();
     int len;                                                         // run length per warp
     uint64_t x[2];
     if (R == 1) {
@@ -438,7 +453,8 @@ struct CtaTopK {
   // End of the scan (every thread calls it): the leftovers of all warps that still beat the threshold are appended
   // to one array (most are stale by now: the threshold rose after they were staged) and warp 0 merges them, 64 at a
   // time -- three barriers, no lock, no queue of eight warps finishing together.
-  __device__ __forceinline__ void cta_drain(uint64_t* scratch, int lane, int warp) {
+  __device__ __forceinline__ void cta_drain(int lane, int warp) {
+    uint64_t* all = scratch();
     const uint64_t t = threshold();
     uint64_t e[3];
     #pragma unroll
@@ -449,24 +465,20 @@ struct CtaTopK {
     }
     __syncthreads();                                                 // leftovers are in registers: the staging area is scratch now
     #pragma unroll
-    for (int c = 0; c < 3; ++c) {
+    for (int c = 0; c < 3; ++c) {                                    // warp_append behind a base reserved from the CTA's counter
       const unsigned m = __ballot_sync(0xffffffffu, e[c] != 0ull);
       if (m) {
         int base = 0;
         if (lane == 0) base = atomicAdd(lock + 1, __popc(m));
         base = __shfl_sync(0xffffffffu, base, 0);
-        if (e[c] != 0ull) scratch[base + __popc(m & ((1u << lane) - 1))] = e[c];
+        if (e[c] != 0ull) all[base + __popc(m & ((1u << lane) - 1))] = e[c];
       }
     }
     __syncthreads();
     if (warp == 0) {
       const int total = *reinterpret_cast<volatile int*>(lock + 1);
-      for (int c0 = 0; c0 < total; c0 += 64) {
-        uint64_t x[2] = {c0 + lane < total ? scratch[c0 + lane] : 0ull, c0 + 32 + lane < total ? scratch[c0 + 32 + lane] : 0ull};
-        reg_sort<2, true>(x, lane);
-        if (kp == 32) { uint64_t y[1] = {x[1]}; warp_merge_run<1>(list, kp, y, lane); }
-        else warp_merge_run<2>(list, kp, x, lane);
-      }
+      for (int c0 = 0; c0 < total; c0 += 64)
+        merge_staged<2>(all + c0, min(total - c0, 64), kp, lane, [&](const auto& x) { warp_merge_run(list, kp, x, lane); });
     }
     cnt = 0;
     __syncthreads();

@@ -222,9 +222,7 @@ centroid_stream_kernel(const float* __restrict__ data, const int64_t* __restrict
       for (int j0 = 0; j0 < k; j0 += 32) {
         const int j = j0 + lane;
         const int c = j < k ? cur[j] : 0;
-        int incl = c;
-        #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+        const int incl = warp_inclusive_scan(c, lane);
         if (j < k) seg[j] = carry + incl - c;
         carry += __shfl_sync(0xffffffffu, incl, 31);
       }

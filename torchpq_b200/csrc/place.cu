@@ -122,8 +122,7 @@ empty_prefix_kernel(const uint8_t* __restrict__ is_empty, int64_t cap, const uin
   uint32_t f[EP_PER], s = 0;
   #pragma unroll
   for (int u = 0; u < EP_PER; ++u) { f[u] = (a0 + u < cap) ? (is_empty[a0 + u] != 0) : 0u; s += f[u]; }
-  uint32_t incl = s;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+  const uint32_t incl = warp_inclusive_scan(s, lane);
   if (lane == 31) wsum[warp] = incl;
   __syncthreads();
   uint32_t before = tile_base[blockIdx.x] + incl - s;

@@ -16,7 +16,8 @@
 //     sub-quantizers, software pipelined one unit ahead (ping-pong register sets).
 //   * top-k (CtaTopK, common.cuh): one compare against the CTA-wide running k-th best + one ballot per
 //     block; survivors are staged per warp and merged into the CTA's single sorted list under a lock;
-//     the threshold is bootstrapped, and the buffers are drained, by CTA-wide sorts.
+//     the threshold is bootstrapped, and the buffers are drained, by CTA-wide sorts.  The selector lays out its own
+//     shared memory (threshold, lock, list, staging buffers): the kernel reserves CtaTopK::bytes and passes the address.
 //   * RES variant: residual IVFPQ (per-cell LUT = query half + precomputed cell half).
 // Sub-quantizer sums are fp32 in four interleaved partial sums (exact for integer LUTs;
 // ~1e-7 relative otherwise -- the reference's m-ascending order lives in scan_ref.cu).
@@ -81,6 +82,13 @@ __device__ __forceinline__ void adc_unit(const uint32_t (&w)[16], const uint32_t
   }
 }
 
+// This lane's key of a block: the four partial sums of adc_unit are added in this association, on top of `base`, and the
+// lane's address is addr0 + lane.  Every key of both scan kernels is formed here, which is what makes the cell-major
+// path's results the query-major kernel's bit for bit.
+__device__ __forceinline__ uint64_t block_key(const float (&acc)[4], float base, uint32_t addr0, int lane) {
+  return make_key(base + ((acc[0] + acc[1]) + (acc[2] + acc[3])), addr0 + lane);
+}
+
 // Per-warp scan state.  regs[2][16] is the ping-pong pair of unit buffers; every index into it is a
 // compile-time constant after unrolling (PAR / SB are template parameters), so it lives in registers.
 template <int MP, int NW>
@@ -123,8 +131,7 @@ struct Scanner {
   __device__ __forceinline__ void process_block(bool has_next) {
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     step<PAR, 0>(acc, has_next);
-    const float score = base + ((acc[0] + acc[1]) + (acc[2] + acc[3]));
-    const uint64_t key = make_key(score, a0_cur + lane);
+    const uint64_t key = block_key(acc, base, a0_cur, lane);
     const bool live = (valid_cur >> lane) & 1u;
     if (PAR == 0) thr = tk.threshold();                  // running k-th best of the CTA
     tk.push(live && key > thr, key, lane);
@@ -143,8 +150,7 @@ struct Scanner {
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     simple_units<0>(acc, B);
     const uint32_t v = __ldg(valid + B);
-    const float score = base + ((acc[0] + acc[1]) + (acc[2] + acc[3]));
-    return ((v >> lane) & 1u) ? make_key(score, a0 + lane) : 0ull;
+    return ((v >> lane) & 1u) ? block_key(acc, base, a0, lane) : 0ull;
   }
   // Blocks are handed out dynamically: `next` is a CTA-wide counter in shared memory.  (A static stripe b = warp,
   // warp + NW, ... left the CTA waiting for its slowest warp -- the warp schedulers favour the oldest warps, so the
@@ -178,7 +184,7 @@ struct Scanner {
   }
 };
 
-struct ScanSmem { size_t lut, part1, seg_blk0, seg_addr0, seg_cell, seg_prefix, thr, lock, rep, list, bufs, total; };
+struct ScanSmem { size_t lut, part1, seg_blk0, seg_addr0, seg_cell, seg_prefix, next, topk, total; };
 static ScanSmem scan_smem(int MP, int n_probe, int nw, int kp, bool residual = false, bool part1_in_smem = false) {
   ScanSmem s; size_t off = 0;
   s.lut = off;        off += lut_bytes(MP);
@@ -187,12 +193,9 @@ static ScanSmem scan_smem(int MP, int n_probe, int nw, int kp, bool residual = f
   s.seg_blk0 = off;   off += (size_t)n_probe * 4;
   s.seg_addr0 = off;  off += (size_t)n_probe * 4;
   s.seg_prefix = off; off += (size_t)(n_probe + 1) * 4;
+  s.next = off;       off += 4;                                       // the block cursor (Scanner::next)
   off = align_up(off, 8);
-  s.thr = off;        off += 8;
-  s.lock = off;       off += 16;                                      // list lock, drain counter, block cursor
-  s.rep = off;        off += (size_t)nw * 8;
-  s.list = off;       off += (size_t)kp * 8;
-  s.bufs = off;       off += (size_t)nw * kStage * 8;
+  s.topk = off;       off += CtaTopK::bytes(nw, kp);
   s.total = off;
   return s;
 }
@@ -282,9 +285,7 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
         seg_addr0[j] = e.addr0;
         if constexpr (RES) seg_cell[j] = (int32_t)e.cell;
       }
-      int incl = nb;
-      #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+      const int incl = warp_inclusive_scan(nb, lane);
       if (j < P) seg_prefix[j + 1] = carry + incl;
       carry += __shfl_sync(0xffffffffu, incl, 31);
     }
@@ -313,10 +314,8 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   Scanner<MP, NW> sc;
   sc.codes = A.codes; sc.valid = A.valid; sc.lut = lut;
   sc.seg_prefix = seg_prefix; sc.seg_blk0 = seg_blk0; sc.seg_addr0 = seg_addr0; sc.lane = lane;
-  sc.next = reinterpret_cast<int*>(smem + L.lock) + 2;
-  sc.tk.init(reinterpret_cast<uint64_t*>(smem + L.list), reinterpret_cast<unsigned long long*>(smem + L.thr),
-             reinterpret_cast<int*>(smem + L.lock), reinterpret_cast<uint64_t*>(smem + L.bufs) + (size_t)warp * kStage,
-             A.kp, A.k);
+  sc.next = reinterpret_cast<int*>(smem + L.next);
+  sc.tk.init(smem + L.topk, NW, warp, A.kp, A.k);
   lane_slot_offsets(sc.off, lane);
   __syncthreads();
   TPQ_PHASE(0);
@@ -327,7 +326,6 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   sc.thr = 0; sc.base = 0.f;
   sc.seg = 0; sc.seg_lo = 0; sc.seg_hi = seg_prefix[1]; sc.seg_b0 = seg_blk0[0]; sc.seg_a0 = seg_addr0[0];
   CtaTopK& tk = sc.tk;
-  uint64_t* bufs = reinterpret_cast<uint64_t*>(smem + L.bufs);
   if constexpr (RES) {
     // query half of the LUT: the shared-memory table built above (DSUB > 0), or the staged copy in global memory
     const float4* p1 = DSUB > 0 ? reinterpret_cast<const float4*>(smem + L.part1)
@@ -348,7 +346,7 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
       sc.base = A.base_sims[(size_t)q * A.n_probe + j];
       sc.run(b1);
     }
-    tk.cta_drain(bufs, lane, warp);
+    tk.cta_drain(lane, warp);
     write_keys<NW>(A, tk.list, q, slice, tid);
     return;
   }
@@ -365,14 +363,14 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
     }
     tk.cnt = R * 32;
 #ifdef TPQ_DEBUG_KNOBS
-    if (A.boot_mode == 1) tk.cta_bootstrap(bufs, NW, R, lane, warp); else
+    if (A.boot_mode == 1) tk.cta_bootstrap(NW, R, lane, warp); else
 #endif
-    tk.cta_quickstart(reinterpret_cast<uint64_t*>(smem + L.rep), NW, R, lane, warp);
+    tk.cta_quickstart(NW, R, lane, warp);
   }
   TPQ_PHASE(1);
   sc.run(b_end);
   TPQ_PHASE(2);
-  tk.cta_drain(bufs, lane, warp);                          // leftovers of all warps: register sorts + merge tree, no lock
+  tk.cta_drain(lane, warp);                                // leftovers of all warps: register sorts + merge tree, no lock
   TPQ_PHASE(3);
 #ifdef TPQ_DEBUG_KNOBS
   if (A.phase && tid == 0) atomicAdd(A.phase + 4, 1ull);
@@ -438,7 +436,7 @@ static int launch_merge(const uint64_t* keys_in, int nq, int n_parts, int k, int
 //   pass 2  ivfpq_cell_scan_kernel over entries 1 .. P-1: every key above the bound is appended to the query's survivors;
 //   select  per query, the top k of the pass-1 list and the survivors (cell_select_kernel).
 // Exact: a candidate that is neither in the pass-1 list nor a survivor is <= the bound, and the pass-1 list already
-// holds k keys >= the bound.  Scores are formed exactly as in the query-major kernel, so results are bit-identical.
+// holds k keys >= the bound.  Both kernels form their keys in block_key, so results are bit-identical.
 constexpr int kCellSlots = 3;         // LUT ring depth (64 KB each)
 constexpr int kCellNW = 12;           // warps of a cell-scan CTA
 constexpr int kCellR = 7;             // code blocks per warp held in registers (168 registers): a chunk is up to 84 blocks = 2688 vectors
@@ -607,8 +605,6 @@ ivfpq_cell_scan_kernel(CellArgs A) {
   // the slot's words.
   // It reads shared memory only: the thread that refills a slot is the last to leave it, and every warp waits for
   // what it waits for here.
-  // It reads shared memory only: the thread that refills a slot is the last to leave it, and every warp waits for
-  // what it waits for here.
   auto issue = [&](int i, int s) {
     const int qi = (int)lds_u32(win_q + 4 * i);
     slot_q[s] = qi;
@@ -659,12 +655,10 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         if (r < nr) {
           float acc[4] = {0.f, 0.f, 0.f, 0.f};
           adc_unit<MP, 0>(w[r], off, lut, acc);
-          const float score = (acc[0] + acc[1]) + (acc[2] + acc[3]);
-          const uint64_t key = make_key(score, a0 + (uint32_t)(ci.b_lo + warp + r * NW) * 32u + lane);
-          const bool pass = ((vmask[r] >> lane) & 1u) && key > thr;
-          const unsigned m = __ballot_sync(0xffffffffu, pass);
-          if (pass) stage[n + __popc(m & ((1u << lane) - 1))] = key;
-          n += __popc(m);
+          // base -0.f: x + -0.f is x, so no add is issued.  The query-major kernel adds +0.f here, which is the same
+          // score: a sum of partial sums that start from +0.f is never -0.f.
+          const uint64_t key = block_key(acc, -0.f, a0 + (uint32_t)(ci.b_lo + warp + r * NW) * 32u, lane);
+          n += warp_append(stage, n, ((vmask[r] >> lane) & 1u) && key > thr, key, lane);
         }
       }
       __syncwarp();

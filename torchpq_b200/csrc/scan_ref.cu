@@ -17,7 +17,7 @@ namespace tpq {
 
 struct RefScanSmem {
   // byte offsets into dynamic shared memory
-  size_t lut, seg_start, seg_size, seg_prefix, thr, lock, list, bufs, total;
+  size_t lut, seg_start, seg_size, seg_prefix, topk, total;
 };
 
 static RefScanSmem ref_scan_smem(int M, int n_probe, int nw, int kp) {
@@ -28,10 +28,7 @@ static RefScanSmem ref_scan_smem(int M, int n_probe, int nw, int kp) {
   s.seg_size = off;   off += (size_t)n_probe * sizeof(int32_t);
   s.seg_prefix = off; off += (size_t)(n_probe + 1) * sizeof(int32_t);
   off = align_up(off, 8);
-  s.thr = off;        off += 8;
-  s.lock = off;       off += 8;
-  s.list = off;       off += (size_t)kp * sizeof(uint64_t);
-  s.bufs = off;       off += (size_t)nw * kStage * sizeof(uint64_t);
+  s.topk = off;       off += CtaTopK::bytes(nw, kp);
   s.total = off;
   return s;
 }
@@ -80,20 +77,13 @@ ivfpq_topk_ref_kernel(const uint32_t* __restrict__ data,        // [M/4, n_data]
         seg_size[j] = (int)n;
         chunks = (int)((n + 31) >> 5);
       }
-      int incl = chunks;
-      #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        int v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += v;
-      }
+      const int incl = warp_inclusive_scan(chunks, lane);
       if (j < P) seg_prefix[j + 1] = carry + incl;
       carry += __shfl_sync(0xffffffffu, incl, 31);
     }
   }
   CtaTopK tk;
-  tk.init(reinterpret_cast<uint64_t*>(smem + L.list), reinterpret_cast<unsigned long long*>(smem + L.thr),
-          reinterpret_cast<int*>(smem + L.lock), reinterpret_cast<uint64_t*>(smem + L.bufs) + (size_t)warp * kStage,
-          kp, k);
+  tk.init(smem + L.topk, nw, warp, kp, k);
   __syncthreads();
 
   const int total_chunks = seg_prefix[P];
