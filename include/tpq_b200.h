@@ -29,9 +29,10 @@ typedef enum {
   TPQ_ERR_CUDA = -4          /* a CUDA runtime call failed (message carries cudaGetErrorString) */
 } tpq_status;
 
-/* MANHATTAN exists for k-means assignment only (tpq_max_sim, tpq_kmeans_assign, exact kernel); every LUT, relayout and
- * search entry point rejects it: the index is defined for euclidean and cosine. */
-enum { TPQ_METRIC_EUCLIDEAN = 0, TPQ_METRIC_COSINE = 1, TPQ_METRIC_MANHATTAN = 2 };
+/* MANHATTAN exists for k-means assignment only (tpq_max_sim, tpq_kmeans_assign, exact kernel) and INNER for the flat
+ * search only (tpq_flat_*); every IVFPQ, LUT and relayout entry point rejects both: the IVFPQ index is defined for
+ * euclidean and cosine. */
+enum { TPQ_METRIC_EUCLIDEAN = 0, TPQ_METRIC_COSINE = 1, TPQ_METRIC_MANHATTAN = 2, TPQ_METRIC_INNER = 3 };
 
 /* Index state read by search.  Field-for-field the buffers of the reference's
  * CellContainer / BaseContainer / codecs (container/CellContainer.py:46-81,
@@ -145,6 +146,23 @@ int tpq_ivfpq_search_cells(const tpq_index* index, const float* x_dn, const int6
                            const int64_t* n_probe_list, int nq, int n_probe, int k,
                            float* values, int64_t* ids, int64_t* address, uint64_t* keys_out,
                            void* ws, size_t ws_bytes, void* stream);
+
+/* ------------------------------------------------------------------ flat (exact brute-force) search
+ * FlatIndex.search (FlatIndex.py:46-101) over base [d, ld] f32 (row stride ld = the store's capacity), columns
+ * [0, n) live, n < 2^32.  Scores, exact fp32 (one fmaf chain over i ascending per dot product):
+ *   EUCLIDEAN ((2 x.b) - |x|^2) - |b|^2      COSINE (x / (|x| + 1e-8)).b / (|b| + 1e-8)      INNER x.b
+ * tpq_flat_norms: the per-column table search reads, norms [n] f32 (|b|^2 squares separately rounded, or |b| + 1e-8;
+ *   nothing for INNER, whose norms may be NULL).  Compute it once per store state.
+ * tpq_flat_search: x_dn [d, nq] -> values [nq, k] f32 descending (-inf padded), ids [nq, k] i64
+ *   (address2id[address], -1 padded), address [nq, k] i64 (nullable, -1 padded).  Order: score descending, then address
+ *   ascending.  The [nq, n] score matrix is never stored: one fused GEMM + top-k kernel, then tpq_merge_topk.
+ *   k > 1024 and metrics other than the three above: TPQ_ERR_UNSUPPORTED.  ws: at least
+ *   tpq_flat_workspace_bytes(d, nq, n, k) bytes (bounded in n). */
+int tpq_flat_norms(const float* base, int64_t ld, int d, int64_t n, int metric, float* norms, void* stream);
+size_t tpq_flat_workspace_bytes(int d, int nq, int64_t n, int k);
+int tpq_flat_search(const float* x_dn, int d, int nq, const float* base, int64_t ld, int64_t n,
+                    const float* norms, int metric, int k, const int64_t* address2id,
+                    float* values, int64_t* ids, int64_t* address, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------ k-means / codec neighbours of the path
  * tpq_max_sim: MultiKMeans assignment, MaxSimCuda(dim=2, mode "tn") (kernels/MaxSimCuda.py:184-238,

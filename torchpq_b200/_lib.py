@@ -20,7 +20,7 @@ TPQ_ERR_UNSUPPORTED = -2
 TPQ_ERR_WORKSPACE = -3
 TPQ_ERR_CUDA = -4
 
-METRIC = {"euclidean": 0, "cosine": 1, "manhattan": 2}   # manhattan: k-means assignment only
+METRIC = {"euclidean": 0, "cosine": 1, "manhattan": 2, "inner": 3}   # manhattan: k-means assignment only; inner: flat search only
 
 
 class TpqIndex(C.Structure):
@@ -78,6 +78,9 @@ SIGNATURES = {
     "tpq_get_write_address": (_I, [_P, _P, _I64, _P, _P, _P, _I, _P, _P, _P]),
     "tpq_store_codes": (_I, [_P, _P, _P, _P, _I64, _IX, _P, _P, _P, _P, _P, _P, _P]),
     "tpq_expand_move": (_I, [_P, _P, _P, _P, _P, _I, _I, _I64, _I64, _P, _P, _P, _P]),
+    "tpq_flat_norms": (_I, [_P, _I64, _I, _I64, _I, _P, _P]),
+    "tpq_flat_workspace_bytes": (_SZ, [_I, _I, _I64, _I]),
+    "tpq_flat_search": (_I, [_P, _I, _I, _P, _I64, _I64, _P, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 

@@ -7,20 +7,21 @@
 //   smart probing                           torchpq/index/IVFPQIndex.py:499-512 (~8 torch launches)
 // with three launches: squared norms, a tiled fp32 GEMM with the "*2 - |x|^2 - |c|^2"
 // epilogue fused, and a warp-per-query top-n_probe select with smart probing fused.
-#include "common.cuh"
+#include "gemm_tile.cuh"
 
 namespace tpq {
 
-// Column reductions over a [d, n] matrix.  A CTA owns 32 columns; its 32 x 32 threads split the rows 32 ways
-// (coalesced 128-byte row segments), partial sums meet in shared memory.  Row-group partials are combined in
-// ascending group order, so the result is deterministic.  (32 row groups rather than round 1's 8: a 1000-query
+// Column reductions over a [d, n] matrix with row stride ld.  A CTA owns 32 columns; its 32 x 32 threads split the
+// rows 32 ways (coalesced 128-byte row segments), partial sums meet in shared memory.  Row-group partials are combined
+// in ascending group order, so the result is deterministic.  (32 row groups rather than round 1's 8: a 1000-query
 // batch is only 32 CTAs, so at d = 960 the per-thread row loop was the whole latency of the cosine step.)
 constexpr int CR_G = 32;    // row groups per CTA
-__device__ __forceinline__ float col_sumsq(const float* __restrict__ x, int d, int n, int j, int g, float (*part)[33], bool fma) {
+__device__ __forceinline__ float col_sumsq(const float* __restrict__ x, int d, int64_t n, int64_t ld, int64_t j, int g,
+                                           float (*part)[33], bool fma) {
   float s = 0.f;
   if (j < n) {
     for (int i = g; i < d; i += CR_G) {
-      const float v = x[(size_t)i * n + j];
+      const float v = x[(size_t)i * ld + j];
       s = fma ? fmaf(v, v, s) : __fadd_rn(s, __fmul_rn(v, v));
     }
   }
@@ -34,90 +35,73 @@ __device__ __forceinline__ float col_sumsq(const float* __restrict__ x, int d, i
 
 // out[j] = sum_i x[i, j]^2   (torch's (a ** 2).sum(dim=-2): separately rounded squares)
 __global__ void __launch_bounds__(32 * CR_G)
-col_sqnorm_kernel(const float* __restrict__ x, int d, int n, float* __restrict__ out) {
+col_sqnorm_kernel(const float* __restrict__ x, int d, int64_t n, int64_t ld, float* __restrict__ out) {
   __shared__ float part[CR_G][33];
-  const int j = blockIdx.x * 32 + (threadIdx.x & 31), g = threadIdx.x >> 5;
-  const float t = col_sumsq(x, d, n, j, g, part, false);
+  const int64_t j = (int64_t)blockIdx.x * 32 + (threadIdx.x & 31);
+  const int g = threadIdx.x >> 5;
+  const float t = col_sumsq(x, d, n, ld, j, g, part, false);
   if (g == 0 && j < n) out[j] = t;
 }
 
-// out[:, j] = x[:, j] / (||x[:, j]||_2 + 1e-9)   (util.py:38-43)
+// out[j] = ||x[:, j]||_2 + eps, the divisor of normalize_columns_kernel
 __global__ void __launch_bounds__(32 * CR_G)
-normalize_columns_kernel(const float* __restrict__ x, int d, int n, float* __restrict__ out) {
+col_norm_kernel(const float* __restrict__ x, int d, int64_t n, int64_t ld, float eps, float* __restrict__ out) {
+  __shared__ float part[CR_G][33];
+  const int64_t j = (int64_t)blockIdx.x * 32 + (threadIdx.x & 31);
+  const int g = threadIdx.x >> 5;
+  const float t = col_sumsq(x, d, n, ld, j, g, part, true);
+  if (g == 0 && j < n) out[j] = __fadd_rn(sqrtf(t), eps);
+}
+
+// out[:, j] = x[:, j] / (||x[:, j]||_2 + eps)   (util.py:38-43 with eps 1e-9; metric.py:14-25 with eps 1e-8)
+__global__ void __launch_bounds__(32 * CR_G)
+normalize_columns_kernel(const float* __restrict__ x, int d, int n, float eps, float* __restrict__ out) {
   __shared__ float part[CR_G][33];
   const int j = blockIdx.x * 32 + (threadIdx.x & 31), g = threadIdx.x >> 5;
-  const float t = col_sumsq(x, d, n, j, g, part, true);
+  const float t = col_sumsq(x, d, n, n, j, g, part, true);
   if (j >= n) return;
-  const float nrm = __fadd_rn(sqrtf(t), 1e-9f);
+  const float nrm = __fadd_rn(sqrtf(t), eps);
   for (int i = g; i < d; i += CR_G) out[(size_t)i * n + j] = __fdiv_rn(x[(size_t)i * n + j], nrm);
 }
 
+static unsigned col_blocks(int64_t n) { return (unsigned)((n + 31) / 32); }
+
+int col_sqnorms(const float* x, int d, int64_t n, int64_t ld, float* out, cudaStream_t st) {
+  if (n == 0) return TPQ_OK;
+  col_sqnorm_kernel<<<col_blocks(n), 32 * CR_G, 0, st>>>(x, d, n, ld, out);
+  TPQ_LAUNCH_CHECK("col_sqnorm_kernel");
+  return TPQ_OK;
+}
+
+int col_norms(const float* x, int d, int64_t n, int64_t ld, float eps, float* out, cudaStream_t st) {
+  if (n == 0) return TPQ_OK;
+  col_norm_kernel<<<col_blocks(n), 32 * CR_G, 0, st>>>(x, d, n, ld, eps, out);
+  TPQ_LAUNCH_CHECK("col_norm_kernel");
+  return TPQ_OK;
+}
+
+int normalize_columns(const float* x, int d, int n, float eps, float* out, cudaStream_t st) {
+  if (n == 0) return TPQ_OK;
+  normalize_columns_kernel<<<col_blocks(n), 32 * CR_G, 0, st>>>(x, d, n, eps, out);
+  TPQ_LAUNCH_CHECK("normalize_columns_kernel");
+  return TPQ_OK;
+}
+
 // sims[q, c] = ((2 * sum_i x[i,q] * cb[i,c]) - xn[q]) - cn[c]        (metric.py:75-94)
-// 128x128 tile, 256 threads, 8x8 micro-tile split in two 4-wide halves so that
-// shared-memory reads are conflict-free float4s; K step 16.
-constexpr int GB = 128, GK = 16;
+// The QT = 128 instance of the GEMM tile: a 128 x 128 tile per CTA.
 __global__ void __launch_bounds__(256)
 coarse_gemm_kernel(const float* __restrict__ x, const float* __restrict__ cb,
                    const float* __restrict__ xn, const float* __restrict__ cn,
                    int d, int nq, int C, float* __restrict__ sims) {
-  // two shared-memory stages; the next K-slab is fetched into registers while the current one is multiplied,
-  // so there is one barrier per slab and the global-load latency hides behind 16 x 64 FMAs per thread
-  __shared__ __align__(16) float As[2][GK][GB];
-  __shared__ __align__(16) float Bs[2][GK][GB];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  using G = GemmTile<GB>;
+  __shared__ __align__(16) G::Stages stages;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int q0 = blockIdx.y * GB, c0 = blockIdx.x * GB;
   float acc[8][8];
-  #pragma unroll
-  for (int i = 0; i < 8; ++i)
-    #pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-
-  float ra[8], rb[8];
-  auto fetch = [&](int k0) {                              // 16 x 128 floats per operand = 8 per thread
-    #pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const int e = r * 256 + tid, kk = e >> 7, col = e & 127, gk = k0 + kk;
-      ra[r] = (gk < d && q0 + col < nq) ? __ldg(x + (size_t)gk * nq + q0 + col) : 0.f;
-      rb[r] = (gk < d && c0 + col < C) ? __ldg(cb + (size_t)gk * C + c0 + col) : 0.f;
-    }
-  };
-  auto stash = [&](int buf) {
-    #pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const int e = r * 256 + tid, kk = e >> 7, col = e & 127;
-      As[buf][kk][col] = ra[r];
-      Bs[buf][kk][col] = rb[r];
-    }
-  };
-  fetch(0);
-  stash(0);
-  __syncthreads();
-  int cur = 0;
-  for (int k0 = 0; k0 < d; k0 += GK) {
-    const bool more = k0 + GK < d;
-    if (more) fetch(k0 + GK);
-    #pragma unroll
-    for (int kk = 0; kk < GK; ++kk) {
-      float4 a0 = *reinterpret_cast<const float4*>(&As[cur][kk][ty * 4]);
-      float4 a1 = *reinterpret_cast<const float4*>(&As[cur][kk][64 + ty * 4]);
-      float4 b0 = *reinterpret_cast<const float4*>(&Bs[cur][kk][tx * 4]);
-      float4 b1 = *reinterpret_cast<const float4*>(&Bs[cur][kk][64 + tx * 4]);
-      float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-      float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-      #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        #pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-    }
-    if (more) {
-      stash(cur ^ 1);                                       // the other stage was last read one iteration ago
-      __syncthreads();
-      cur ^= 1;
-    }
-  }
+  G::run(x, nq, q0, cb + c0, C, C - c0, d, stages, acc);
   #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    int q = q0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
+    int q = q0 + G::row(i, ty);
     if (q >= nq) continue;
     float a2 = xn[q];
     #pragma unroll
@@ -221,10 +205,7 @@ using namespace tpq;
 
 extern "C" int tpq_normalize_columns(const float* x_dn, int d, int nq, float* out_dn, void* stream) {
   TPQ_REQUIRE(x_dn && out_dn && d > 0 && nq >= 0, "tpq_normalize_columns: bad argument");
-  if (nq == 0) return TPQ_OK;
-  normalize_columns_kernel<<<(nq + 31) / 32, 32 * CR_G, 0, (cudaStream_t)stream>>>(x_dn, d, nq, out_dn);
-  TPQ_LAUNCH_CHECK("normalize_columns_kernel");
-  return TPQ_OK;
+  return normalize_columns(x_dn, d, nq, 1e-9f, out_dn, (cudaStream_t)stream);
 }
 
 extern "C" size_t tpq_coarse_workspace_bytes(int d, int nq, int n_cells) {
@@ -250,8 +231,8 @@ extern "C" int tpq_coarse_probe(const float* x_dn, const float* vq_codebook, int
   float* sims = reinterpret_cast<float*>(w);  w += align_up((size_t)nq * n_cells * 4, 256);
   float* xn = reinterpret_cast<float*>(w);    w += align_up((size_t)nq * 4, 256);
   float* cn = reinterpret_cast<float*>(w);
-  col_sqnorm_kernel<<<(nq + 31) / 32, 32 * CR_G, 0, st>>>(x_dn, d, nq, xn);
-  col_sqnorm_kernel<<<(n_cells + 31) / 32, 32 * CR_G, 0, st>>>(vq_codebook, d, n_cells, cn);
+  if (int rc = col_sqnorms(x_dn, d, nq, nq, xn, st)) return rc;
+  if (int rc = col_sqnorms(vq_codebook, d, n_cells, n_cells, cn, st)) return rc;
   dim3 grid((n_cells + GB - 1) / GB, (nq + GB - 1) / GB);
   coarse_gemm_kernel<<<grid, 256, 0, st>>>(x_dn, vq_codebook, xn, cn, d, nq, n_cells, sims);
   TPQ_LAUNCH_CHECK("coarse_gemm_kernel");

@@ -18,7 +18,7 @@ import torch
 
 from . import _lib
 from ._lib import lib, check, ptr
-from .modules import StateModule, Codec
+from .modules import Codec, IdContainer, _fingerprint
 
 
 def _codebook_of(codec):
@@ -27,10 +27,6 @@ def _codebook_of(codec):
     km = getattr(codec, "kmeans", None)
     cb = getattr(km, "centroids", None) if km is not None else None
     return cb if cb is not None else codec.codebook
-
-
-def _fingerprint(*tensors):
-    return tuple((t.data_ptr(), t._version, tuple(t.shape)) if t is not None else None for t in tensors)
 
 
 class ScanLayout:
@@ -118,7 +114,7 @@ class ScanLayout:
         return sum(t.numel() * t.element_size() for t in ts if t is not None)
 
 
-class IVFPQIndex(StateModule):
+class IVFPQIndex(IdContainer):
     def __init__(self, d_vector, n_subvectors=8, n_cells=128, initial_size=None, expand_step_size=128,
                  expand_mode="double", distance="euclidean", device="cuda:0", pq_use_residual=False, verbose=0):
         super().__init__()
@@ -166,14 +162,6 @@ class IVFPQIndex(StateModule):
 
     # ------------------------------------------------------------------ container properties
     @property
-    def capacity(self):
-        return self._address2id.shape[0]
-
-    @property
-    def max_id(self):
-        return self._max_id
-
-    @property
     def n_items(self):
         assert self._is_empty is not None, "shard-only index (dist.distribute) keeps no per-slot state"
         return int((self._is_empty == 0).sum().item())               # live vectors (== _cell_size.sum() until a remove)
@@ -193,11 +181,6 @@ class IVFPQIndex(StateModule):
         super().load_state_dict(state_dict, strict)
         self._has_holes = True                                          # unknown provenance: assume the container may have holes
         self._refresh_max_id()
-
-    def _refresh_max_id(self):
-        a2i = self._address2id
-        self._max_id = int(a2i.max().item()) if a2i is not None and a2i.numel() else -1
-        self._id2address_fp = None
 
     # ------------------------------------------------------------------ state import
     def load_state(self, st):
@@ -350,26 +333,6 @@ class IVFPQIndex(StateModule):
         from . import build
         return build.add(self, x, ids, return_address)
 
-    def get_address_by_id(self, ids):
-        """BaseContainer.get_address_by_id with the inverse id map (BaseContainer.py:78-110; IVFPQIndex builds its
-        container with use_inverse_id_mapping=True, IVFPQIndex.py:39)."""
-        assert ids.dtype == torch.int64
-        ids = ids.to(self._address2id.device)
-        if self._id2address is None or self._id2address_fp != _fingerprint(self._address2id):
-            a2i_v, a2i_i = self._address2id.sort()
-            keep = a2i_v >= 0
-            if a2i_v.numel():                                          # never trust a stale _max_id (checkpoint loads)
-                self._max_id = max(self._max_id, int(a2i_v[-1].item()))
-            id2a = -torch.ones(self._max_id + 1, dtype=torch.long, device=ids.device)
-            id2a[a2i_v[keep]] = a2i_i[keep]
-            delattr(self, "_id2address")
-            self.register_buffer("_id2address", id2a)
-            self._id2address_fp = _fingerprint(self._address2id)
-        mask = (0 <= ids) & (ids <= self._max_id)
-        address = torch.ones_like(ids) * -1
-        address[mask] = self._id2address[ids[mask]]
-        return address
-
     def remove(self, ids=None, address=None):
         """CellContainer.remove (CellContainer.py:369-393) as it is documented to behave (README.md:60-66: "virtually
         remove vectors ... ignores ids that don't exist").  The shipped reference returns early whenever fewer items
@@ -419,11 +382,3 @@ class IVFPQIndex(StateModule):
             return self.vq_codec.codebook[:, vq_code] + fn.pq_decode(self.pq_codec.codebook, pq_code)
         assert len(code.shape) == 2 and code.shape[0] == self.n_subvectors
         return fn.pq_decode(self.pq_codec.codebook, code)
-
-    def get_id_by_address(self, address):
-        """BaseContainer.get_id_by_address (BaseContainer.py:58-65) -- plain tensor indexing, not on the hot path."""
-        assert address.dtype == torch.int64
-        mask = (0 <= address) & (address < self.capacity)
-        ids = torch.ones_like(address) * -1
-        ids[mask] = self._address2id[address[mask]]
-        return ids

@@ -35,6 +35,59 @@ class StateModule(nn.Module):
         pass
 
 
+def _fingerprint(*tensors):
+    return tuple((t.data_ptr(), t._version, tuple(t.shape)) if t is not None else None for t in tensors)
+
+
+class IdContainer(StateModule):
+    """The id bookkeeping of BaseContainer (container/BaseContainer.py:30-110) that IVFPQIndex and FlatIndex share: the
+    ``_address2id`` / ``_id2address`` buffers, ``capacity``, ``max_id`` (tracked, and re-derived from ``_address2id``
+    after a checkpoint load, where the reference restarts it at -1) and the two lookups.  The inverse map is rebuilt
+    lazily, whenever ``_address2id`` has changed since it was built.  Subclasses register both buffers and set
+    ``_max_id = -1`` and ``_id2address_fp = None``."""
+
+    @property
+    def capacity(self):
+        return self._address2id.shape[0]
+
+    @property
+    def max_id(self):
+        return self._max_id
+
+    def _refresh_max_id(self):
+        a2i = self._address2id
+        self._max_id = int(a2i.max().item()) if a2i is not None and a2i.numel() else -1
+        self._id2address_fp = None
+
+    def get_id_by_address(self, address):
+        """BaseContainer.get_id_by_address (BaseContainer.py:58-65) -- plain tensor indexing, not on the hot path."""
+        assert address.dtype == torch.int64
+        mask = (0 <= address) & (address < self.capacity)
+        ids = torch.ones_like(address) * -1
+        ids[mask] = self._address2id[address[mask]]
+        return ids
+
+    def get_address_by_id(self, ids):
+        """BaseContainer.get_address_by_id with the inverse id map (BaseContainer.py:78-110; both indexes build their
+        container with use_inverse_id_mapping=True, IVFPQIndex.py:39, FlatIndex.py:27)."""
+        assert ids.dtype == torch.int64
+        ids = ids.to(self._address2id.device)
+        if self._id2address is None or self._id2address_fp != _fingerprint(self._address2id):
+            a2i_v, a2i_i = self._address2id.sort()
+            keep = a2i_v >= 0
+            if a2i_v.numel():                                          # never trust a stale _max_id (checkpoint loads)
+                self._max_id = max(self._max_id, int(a2i_v[-1].item()))
+            id2a = -torch.ones(self._max_id + 1, dtype=torch.long, device=ids.device)
+            id2a[a2i_v[keep]] = a2i_i[keep]
+            delattr(self, "_id2address")
+            self.register_buffer("_id2address", id2a)
+            self._id2address_fp = _fingerprint(self._address2id)
+        mask = (0 <= ids) & (ids <= self._max_id)
+        address = torch.ones_like(ids) * -1
+        address[mask] = self._id2address[ids[mask]]
+        return address
+
+
 class _Centroids(StateModule):
     """Stands where the reference has KMeans / MultiKMeans: owner of the ``centroids`` buffer
     (clustering/KMeans.py:74, clustering/MultiKMeans.py:73)."""
