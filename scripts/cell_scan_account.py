@@ -11,7 +11,8 @@ search, so they are switched inside one process):
   * runs one more step with the phase buffer set and reads the kernel's cycle account: each phase's share of all
     warps' cycles from kernel entry to exit.
 Configurations: the product shape 12x7; TPQ_CELL_ABLATE=1 (no refills: every pair of an item reuses the first three
-LUTs, which leaves the scoring time of this kernel shape), =2 (no survivors: the reservation never runs), =3 (both);
+LUTs, which leaves the scoring time of this kernel shape), =2 (no survivors: neither the pair tail nor the window
+flush runs), =3 (both);
 TPQ_CELL_CFG=14x6 and 16x5.  The ablations give WRONG search results on purpose; only their times mean anything.
 Writes DIR/cell_scan_account_<workload>.json and prints one line per configuration.
 """
@@ -29,7 +30,7 @@ import torch  # noqa: E402
 import bench  # noqa: E402
 import torchpq_b200 as T  # noqa: E402
 
-PHASES = ("item_prologue", "mbar_wait", "scoring", "release_issue", "reserve_copy_out")
+PHASES = ("item_prologue", "mbar_wait", "scoring", "release_issue", "pair_tail", "window_flush")
 CONFIGS = (("12x7", {}), ("12x7 no refills", {"TPQ_CELL_ABLATE": "1"}), ("12x7 no survivors", {"TPQ_CELL_ABLATE": "2"}),
            ("12x7 no refills, no survivors", {"TPQ_CELL_ABLATE": "3"}),
            ("14x6", {"TPQ_CELL_CFG": "14x6"}), ("16x5", {"TPQ_CELL_CFG": "16x5"}))
@@ -89,8 +90,8 @@ def main():
             torch.cuda.synchronize(dev)
             set_phase(ctypes.c_void_p(0))
             p = phase.cpu().tolist()[8:]
-            total = max(1, p[6])
-            row = {"config": tag, "cell_scan_kernel_ms": kern_ms, "warps": p[5], "cycles_per_warp": total / max(1, p[5]),
+            total = max(1, p[7])
+            row = {"config": tag, "cell_scan_kernel_ms": kern_ms, "warps": p[6], "cycles_per_warp": total / max(1, p[6]),
                    "phase_share": {n: p[j] / total for j, n in enumerate(PHASES)}}
             rows.append(row)
             print(json.dumps(row), flush=True)

@@ -442,18 +442,25 @@ constexpr int kCellNW = 12;           // warps of a cell-scan CTA
 constexpr int kCellR = 7;             // code blocks per warp held in registers (168 registers): a chunk is up to 84 blocks = 2688 vectors
 constexpr int kCellWin = 256;         // pairs of an item whose (query, bound) records sit in shared memory at a time
 // Dynamic shared memory of a cell-scan CTA: the ring, 256 B of barriers and slot state, the warps' survivor stages, then
-// the record window (kCellWin bounds, kCellWin queries).
+// the record window (kCellWin bounds, kCellWin queries, kCellWin survivor counts, kCellWin reserved bases).
 constexpr size_t cell_win_offset(int nw, int r) { return (size_t)kCellSlots * lut_bytes(64) + 256 + (size_t)nw * r * 32 * 8; }
-constexpr size_t cell_smem_bytes(int nw, int r) { return cell_win_offset(nw, r) + (size_t)kCellWin * 12; }
+constexpr size_t cell_smem_bytes(int nw, int r) { return cell_win_offset(nw, r) + (size_t)kCellWin * 20; }
+// Survivor log of a cell-scan CTA: one bucket per pair of the window, each as large as a chunk's keys can be.
+constexpr size_t cell_log_keys(int nw, int r) { return (size_t)kCellWin * nw * r * 32; }
 
 // Shared-memory accesses of the record window, by 32-bit shared address.  The window is kept apart from the pointers the
-// compiler derives from the kernel's shared base, and the pair body keeps reading its query and bound from the slot's
-// fixed words: indexed reads of the window in the pair body made ptxas move that base from a uniform register into a
+// compiler derives from the kernel's shared base, and the pair body keeps reading its bound from the slot's fixed word
+// (its only indexed access is the atomic on its survivor count, through these opaque addresses): indexed reads of the window in the pair body made ptxas move that base from a uniform register into a
 // vector register and add it to every lookup's address (4.2 instead of 3.3 instructions per lookup, sass_census.py).
 __device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
 __device__ __forceinline__ uint64_t lds_u64(uint32_t a) { uint64_t v; asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory"); return v; }
 __device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void sts_u64(uint32_t a, uint64_t v) { asm volatile("st.shared.u64 [%0], %1;" :: "r"(a), "l"(v) : "memory"); }
+__device__ __forceinline__ uint32_t atoms_add_u32(uint32_t a, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.shared.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(a), "r"(v) : "memory");
+  return old;
+}
 constexpr int kCellBuckets = 128;     // work classes of the largest-first item order (4 per octave)
 
 struct CellItem { int32_t cell, b_lo, b_hi, pad; };   // blocks [b_lo, b_hi) of the cell (relative to its first block)
@@ -467,11 +474,13 @@ struct CellArgs {
   const CellItem* items; const int* n_items; int* cursor;
   const uint64_t* keys;           // [nq][k] pass-1 lists; key k-1 is the query's bound
   uint64_t* surv; int* surv_cnt;  // [n][cap] survivors, [n] their count (> cap: overflow), by chunk-local query
+  uint64_t* log;                  // [gridDim.x][kCellWin][NW * R * 32]: each CTA's survivors of a window, by pair
   int q_base, k, cap;
 #ifdef TPQ_DEBUG_KNOBS
   unsigned long long* phase;      // the phase buffer's [8..15]: warp-cycles summed over all warps in item prologue (barrier,
-                                  // code loads, first LUT wait), mbar_wait, scoring, release + issue, reservation + copy-out;
-                                  // [13] = warps, [14] = their cycles from kernel entry to exit
+                                  // code loads, first LUT wait), mbar_wait, scoring, release + issue, pair tail (shared
+                                  // reservation + log copy), window flush; [14] = warps, [15] = their cycles from kernel
+                                  // entry to exit
   int ablate;                     // WRONG RESULTS, to bound a gain: bit 0 = no refills (every pair of an item reuses the
                                   // first kCellSlots LUTs), bit 1 = no survivors (thr = ~0)
 #endif
@@ -562,6 +571,9 @@ __global__ void __launch_bounds__(1024) cell_plan_kernel(const int* __restrict__
 // scoring is the query-major kernel's adc_unit, so a key is the same bit for bit.  Each lookup is PRMT + LDS + FADD, as
 // in the query-major kernel: the pair body is compiled once per ring slot, so the slot's offset is an LDS immediate
 // and the shared-window base a uniform register (scripts/sass_census.py counts it).
+// Survivors leave in two steps.  A warp appends its keys of pair i to bucket i of the CTA's log at an offset from a
+// shared-memory count, with stores that return nothing.  After the window's last pair, the CTA reserves each pair's
+// place in its query's survivor list with one global atomic per pair, all issued together, and copies the buckets there.
 template <int NW, int R>
 __global__ void __launch_bounds__(NW * 32, 1)
 ivfpq_cell_scan_kernel(CellArgs A) {
@@ -570,19 +582,22 @@ ivfpq_cell_scan_kernel(CellArgs A) {
   uint8_t* ring = smem;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kCellSlots * lut_bytes(64));
   uint64_t* slot_thr = full + kCellSlots;
-  int* slot_q = reinterpret_cast<int*>(slot_thr + kCellSlots);
-  int* rel = slot_q + kCellSlots;                              // warps done with the slot's current LUT
+  int* rel = reinterpret_cast<int*>(slot_thr + kCellSlots);   // warps done with the slot's current LUT
   int* item_sh = rel + kCellSlots;                             // [2]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   uint64_t* stage = reinterpret_cast<uint64_t*>(smem + kCellSlots * lut_bytes(64) + 256) + (size_t)warp * R * 32;
   uint32_t win_thr = smem_u32(smem + cell_win_offset(NW, R));
   asm volatile("" : "+r"(win_thr));                            // from here on just a number to the compiler (see lds_u32)
   const uint32_t win_q = win_thr + kCellWin * 8;
+  const uint32_t win_cnt = win_q + kCellWin * 4;               // survivors of each pair of the window, in its log bucket
+  const uint32_t win_base = win_cnt + kCellWin * 4;            // their place in the query's survivor list
+  constexpr int kBucket = NW * R * 32;                         // a chunk's keys: a bucket never overflows
   static_assert(kCellWin <= NW * 32, "one thread per record of the window");
   if (tid == 0) {
     for (int s = 0; s < kCellSlots; ++s) { mbar_init(&full[s], 1); rel[s] = 0; }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  if (tid < kCellWin) sts_u32(win_cnt + 4 * tid, 0u);         // the item loop's first barrier publishes it
 #ifdef TPQ_DEBUG_KNOBS
   // per-warp cycle account, kept in shared memory behind the stages (the kernel has no registers to spare)
   unsigned long long* acct = reinterpret_cast<unsigned long long*>(smem + cell_smem_bytes(NW, R)) + warp * 8;
@@ -601,13 +616,12 @@ ivfpq_cell_scan_kernel(CellArgs A) {
 #endif
   uint32_t off[8];
   lane_slot_offsets(off, lane);
-  // one thread: LUT of pair i of the window into slot s (every warp has released the slot), its query and bound into
-  // the slot's words.
+  // one thread: LUT of pair i of the window into slot s (every warp has released the slot), its bound into the slot's
+  // word.
   // It reads shared memory only: the thread that refills a slot is the last to leave it, and every warp waits for
   // what it waits for here.
   auto issue = [&](int i, int s) {
     const int qi = (int)lds_u32(win_q + 4 * i);
-    slot_q[s] = qi;
     slot_thr[s] = lds_u64(win_thr + 8 * i);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the warps' reads of the slot precede the TMA write
     mbar_expect_tx(&full[s], lut_bytes(64));
@@ -646,7 +660,6 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         parity ^= 1u << s;
       }
       TPQ_CELL_PHASE(i == 0 ? 0 : 1);
-      const int qi = slot_q[s];
       const uint64_t thr = no_surv ? ~0ull : slot_thr[s];
       const uint8_t* lut = ring + s * lut_bytes(64);
       int n = 0;
@@ -672,17 +685,64 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         }
       }
       TPQ_CELL_PHASE(3);
-      if (n) {
-        int base = 0;
-        if (lane == 0) base = atomicAdd(A.surv_cnt + qi, n);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base + n <= A.cap) {
-          uint64_t* dst = A.surv + (size_t)qi * A.cap + base;
-          for (int j = lane; j < n; j += 32) dst[j] = stage[j];
-        }
+      if (n) {                                                 // into bucket i of the log; the window's flush reserves
+        // the first 32 staged keys are read before the count is, so the two shared-memory round trips overlap
+        const uint64_t k0 = lane < n ? stage[lane] : 0ull;
+        uint32_t o = 0;
+        if (lane == 0) o = atoms_add_u32(win_cnt + 4 * i, (uint32_t)n);
+        o = __shfl_sync(0xffffffffu, o, 0);
+        uint64_t* dst = A.log + ((size_t)blockIdx.x * kCellWin + i) * kBucket + o;
+        if (lane < n) dst[lane] = k0;
+        for (int j = lane + 32; j < n; j += 32) dst[j] = stage[j];
         __syncwarp();
       }
       TPQ_CELL_PHASE(4);
+    };
+    // After the window's last pair: one global atomic per pair with survivors reserves the pair's place in its query's
+    // list, and the warps copy each bucket there unless its query has overflowed (surv_cnt ends at the same sum
+    // whatever the order, so the same queries overflow).  The counts are zeroed for the next window.
+    auto flush = [&](int nwin) {
+      __syncthreads();                                         // every count final, every log store visible to the CTA
+      if (tid < nwin) {
+        const uint32_t c = lds_u32(win_cnt + 4 * tid);
+        if (c) {
+          const int b = atomicAdd(A.surv_cnt + lds_u32(win_q + 4 * tid), (int)c);
+          if (b + (int)c <= A.cap) sts_u32(win_base + 4 * tid, (uint32_t)b);
+          else sts_u32(win_cnt + 4 * tid, 0u);                 // overflowed: nothing to copy
+        }
+      }
+      __syncthreads();
+      // Warp w copies buckets w, w + NW, ...: the first 64 keys of U buckets are loaded before any is stored, so a warp
+      // waits for U buckets' reads at once (at C3 a bucket holds about 60 keys).  The first bucket is broadcast from
+      // lane 0, as nr is: a loop the compiler cannot prove warp-uniform leaves the next window's pair bodies possibly
+      // diverged, and ptxas then adds the shared base to every lookup (4.2 instead of 3.35 instructions per lookup,
+      // sass_census.py).
+      constexpr int U = 2;
+      for (int t0 = __shfl_sync(0xffffffffu, warp, 0); t0 < nwin; t0 += U * NW) {
+        uint32_t c[U];
+        uint64_t v[U][2];
+        #pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int t = t0 + u * NW;
+          c[u] = t < nwin ? lds_u32(win_cnt + 4 * t) : 0u;
+          const uint64_t* src = A.log + ((size_t)blockIdx.x * kCellWin + t) * kBucket;
+          v[u][0] = lane < c[u] ? src[lane] : 0ull;
+          v[u][1] = lane + 32 < c[u] ? src[lane + 32] : 0ull;
+        }
+        #pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int t = t0 + u * NW;
+          if (c[u] == 0) continue;
+          const uint64_t* src = A.log + ((size_t)blockIdx.x * kCellWin + t) * kBucket;
+          uint64_t* dst = A.surv + (size_t)lds_u32(win_q + 4 * t) * A.cap + lds_u32(win_base + 4 * t);
+          if (lane < c[u]) dst[lane] = v[u][0];
+          if (lane + 32 < c[u]) dst[lane + 32] = v[u][1];
+          for (uint32_t j = lane + 64; j < c[u]; j += 32) dst[j] = src[j];
+          __syncwarp();
+          if (lane == 0) sts_u32(win_cnt + 4 * t, 0u);
+        }
+      }
+      TPQ_CELL_PHASE(5);
     };
     static_assert(kCellSlots == 3, "one pair body per ring slot");
     for (int p0 = 0; p0 < np; p0 += kCellWin) {
@@ -702,14 +762,15 @@ ivfpq_cell_scan_kernel(CellArgs A) {
         if (i + 1 < nwin) pair(std::integral_constant<int, 1>(), i + 1, nwin);
         if (i + 2 < nwin) pair(std::integral_constant<int, 2>(), i + 2, nwin);
       }
+      if (!no_surv) flush(nwin);                               // no survivors: every count is 0
     }
   }
 #ifdef TPQ_DEBUG_KNOBS
   cell_mark(0);                                                // the wait at the last barrier
   if (A.phase && lane == 0) {
-    for (int ph = 0; ph < 5; ++ph) atomicAdd(A.phase + ph, acct[ph]);
-    atomicAdd(A.phase + 5, 1ull);
-    atomicAdd(A.phase + 6, (unsigned long long)((uint32_t)clock() - t_in));
+    for (int ph = 0; ph < 6; ++ph) atomicAdd(A.phase + ph, acct[ph]);
+    atomicAdd(A.phase + 6, 1ull);
+    atomicAdd(A.phase + 7, (unsigned long long)((uint32_t)clock() - t_in));
   }
 #endif
 #undef TPQ_CELL_PHASE
@@ -771,7 +832,7 @@ static int cell_cap(int k) { return k * 8 > 8192 ? k * 8 : 8192; }
 
 struct SearchWs {
   size_t coarse, probe_sims, cells, npl, xnorm, lut, keys;
-  size_t cell_cnt, cell_off, slot, pair_q, items, ones, surv, surv_cnt;   // cell-major scan only
+  size_t cell_cnt, cell_off, slot, pair_q, items, ones, surv, surv_cnt, cell_log;   // cell-major scan only
   size_t total;
 };
 
@@ -786,6 +847,7 @@ struct ScanPlan {
   int MP, NW, MINB;               // the query-major kernel: ivfpq_scan_kernel<MP, NW, MINB, qm_dsub(), residual>
   int boot_r;                     // blocks per warp in the kernel's bootstrap
   int cell_nw, cell_r;            // the cell-major kernel: ivfpq_cell_scan_kernel<cell_nw, cell_r>
+  int cell_ctas;                  // its persistent CTAs, one per SM; each has a survivor log in the workspace
 #ifdef TPQ_DEBUG_KNOBS
   int boot_mode; unsigned long long* phase;
   int cell_ablate;
@@ -817,6 +879,8 @@ static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, const
   w.ones = off;       off += align_up(cm ? (size_t)nq * 8 : 0, 256);
   w.surv = off;       off += align_up(cm ? (size_t)P.chunk * cell_cap(k) * 8 : 0, 256);
   w.surv_cnt = off;   off += align_up(cm ? (size_t)P.chunk * 4 : 0, 256);
+  // 5.5 MB per CTA at 12 x 7 (726 MB at 132 SMs): sized by the SM count, not by the batch
+  w.cell_log = off;   off += align_up(cm ? (size_t)P.cell_ctas * cell_log_keys(P.cell_nw, P.cell_r) * 8 : 0, 256);
   w.total = off;
   return w;
 }
@@ -832,6 +896,7 @@ static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool 
   P.MP = ix->m_pad;
   P.boot_r = 2;
   P.cell_nw = kCellNW; P.cell_r = kCellR;
+  P.cell_ctas = device_sm_count();
   // LUT source: built inside the scan CTA when d/M is 1, 2, 4 or 8 (the codebook slice a CTA reads from L2, M*dsub KB,
   // is then small next to the codes it goes on to stream: C4, d/M = 8, reads 0.98 MB of codebook per 7.5 MB of codes
   // and saves the 2 x 128 KB LUT round trip through HBM plus one launch); staged through HBM by lut_kernel
@@ -1034,11 +1099,12 @@ static int cell_stage(const ScanPlan& P, const ScanJob& J, ScanKernel qmajor, Sc
   CA.codes = ix->codes_scan; CA.valid = ix->block_valid; CA.cell_block_start = ix->cell_block_start;
   CA.cell_start = ix->cell_start; CA.lut_scan = lut_ws; CA.cell_off = cell_off; CA.cell_cnt = cell_cnt; CA.pair_q = pair_q;
   CA.items = items; CA.n_items = n_items; CA.cursor = n_items + 1; CA.keys = keys; CA.surv = surv; CA.surv_cnt = surv_cnt;
+  CA.log = reinterpret_cast<uint64_t*>(w + W.cell_log);
   CA.q_base = q0; CA.k = J.k; CA.cap = cap;
 #ifdef TPQ_DEBUG_KNOBS
   CA.phase = P.phase ? P.phase + 8 : nullptr; CA.ablate = P.cell_ablate;
 #endif
-  cscan<<<device_sm_count(), P.cell_nw * 32, cs_smem, st>>>(CA);
+  cscan<<<P.cell_ctas, P.cell_nw * 32, cs_smem, st>>>(CA);
   TPQ_LAUNCH_CHECK("ivfpq_cell_scan_kernel");
   cell_select_kernel<<<(n + 3) / 4, 128, sel_smem, st>>>(keys, surv, surv_cnt, q0, n, J.k, kp, cap);
   TPQ_LAUNCH_CHECK("cell_select_kernel");
