@@ -46,7 +46,7 @@ typedef struct tpq_index {
   int64_t capacity;          /* address slots = _address2id.shape[0] */
   const float*   vq_codebook;   /* [d, C]        vq_codec.codebook */
   const float*   pq_codebook;   /* [M, d/M, 256] pq_codec.codebook */
-  const uint8_t* storage;       /* [M/4, capacity, 4] _storage (may be NULL once the scan layout exists) */
+  const uint8_t* storage;       /* [code_size/4, capacity, 4] _storage (may be NULL once the scan layout exists) */
   const uint8_t* is_empty;      /* [capacity] _is_empty */
   const int64_t* cell_start;    /* [C] _cell_start */
   const int64_t* cell_size;     /* [C] _cell_size */
@@ -65,7 +65,10 @@ typedef struct tpq_index {
   /* ---- residual IVFPQ (pq_use_residual=True, IVFPQIndex.py:48-55,160-170); NULL / 0 otherwise ---- */
   const float*    part2_scan;       /* [C, m_pad/64 groups, 256, 64]: -2 <c_cell,m , p_m,code> - |p_m,code|^2 in LUT layout */
   int32_t         residual;         /* 1 = codes are PQ codes of x - vq_centroid(cell) */
-  int32_t         reserved1;
+  /* ---- bytes of code per item in storage: 0 means n_subvectors.  IVFPQRIndex stores M + Mr (its re-rank code after
+   *      the scanned one); the scan, relayout and search read only the first M/4 word planes.  Only tpq_store_codes
+   *      reads this field: it writes code_size/4 planes and puts the first M/4 in the scan layout. ---- */
+  int32_t         code_size;
 } tpq_index;
 
 /* ------------------------------------------------------------------ misc */
@@ -164,6 +167,25 @@ int tpq_flat_search(const float* x_dn, int d, int nq, const float* base, int64_t
                     const float* norms, int metric, int k, const int64_t* address2id,
                     float* values, int64_t* ids, int64_t* address, void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ re-rank (IVFPQRIndex.search, second pass)
+ * candidates [nq, k1] i64: the first pass's addresses (-1 = none), k <= k1 <= 1024.  storage [(M + Mr)/4, capacity, 4]
+ * u8 as tpq_index.storage with code_size = M + Mr: bytes 0..M-1 of an item are its first-level code, M..M+Mr-1 its
+ * re-rank code.  pq_codebook [M, d/M, 256] (read only when use_residual; may be NULL otherwise), pq_rerank_codebook
+ * [Mr, d/Mr, 256].  Per candidate, exactly in fp32:
+ *   y_e = y2_e + y1_e (use_residual) or y2_e, y1 / y2 the first-level / re-rank codebook entries of its codes;
+ *   EUCLIDEAN acc = fmaf(-dif, dif, acc), dif = x_e - y_e, e ascending from +0 (tpq_max_sim's arithmetic);
+ *   COSINE    acc = fmaf(x_e, y_e, acc) on x / (||x|| + 1e-9) (as tpq_normalize_columns), y not normalised;
+ * i.e. the value equals tpq_max_sim(x_q, decoded candidate).  -> values [nq, k] f32 descending (-inf padded), ids
+ * [nq, k] i64 (address2id[address], -1 padded), address [nq, k] i64 (nullable, -1 padded); order score descending,
+ * then address ascending.  Arguments are checked before any launch; nq == 0 returns at once.  ws: at least
+ * tpq_rerank_workspace_bytes(d, nq, k) bytes. */
+size_t tpq_rerank_workspace_bytes(int d, int nq, int k);
+int tpq_rerank(const float* x_dn, int d, int nq, const int64_t* candidates, int k1,
+               const uint8_t* storage, int64_t capacity, int M, int Mr,
+               const float* pq_codebook, const float* pq_rerank_codebook, int use_residual, int metric,
+               int k, const int64_t* address2id, float* values, int64_t* ids, int64_t* address,
+               void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------ k-means / codec neighbours of the path
  * tpq_max_sim: MultiKMeans assignment, MaxSimCuda(dim=2, mode "tn") (kernels/MaxSimCuda.py:184-238,
  *   kernels/cuda/max_sim.cu:182-309; caller clustering/MultiKMeans.py:314-333):
@@ -214,8 +236,11 @@ int tpq_pq_decode(const float* codebook, const uint8_t* code, int M, int dsub, i
  * tpq_get_write_address: the ioa-th empty slot of the item's cell (kernels/cuda/get_write_address_v2.cu:9-41);
  *   empty_prefix == NULL asserts "no holes": the empties of a cell are [start + size, start + capacity).  -1 = no room.
  * tpq_store_codes: set_data_by_address (CellContainer.py:213-239) + address2id / is_empty / cell_size updates
- *   (:354-360; cell_size becomes max(old, slot + 1)).  codes [M, n] u8.  If codes_scan / block_valid (the scan layout of
- *   `index`, non-const here) are given they are updated in place, so the layout stays valid after the add.
+ *   (:354-360; cell_size becomes max(old, slot + 1)).  codes [code_size, n] u8 (index->code_size, 0 = n_subvectors;
+ *   else a multiple of 4 >= n_subvectors, checked before the launch).  If codes_scan / block_valid (the scan layout of
+ *   `index`, non-const here) are given they are updated in place with the first n_subvectors code bytes, so the layout
+ *   stays valid after the add.
+ * tpq_expand_move's M is the number of code bytes per item (code_size), i.e. storage holds M/4 word planes.
  * tpq_expand_move: CellContainer.expand (:249-311) for many cells at once: every old slot a moves to a + shift[cell(a)];
  *   the caller pre-fills the new buffers (storage 0, address2id -1, is_empty 1) and updates the per-cell tables. */
 size_t tpq_ioa_workspace_bytes(int64_t n, int n_cells);

@@ -1,14 +1,15 @@
-"""torchpq_b200 -- H100-native (sm_90a) IVFPQ search path behind torchpq.index.IVFPQIndex.search(), exact flat search
-(FlatIndex), and k-means (clustering.KMeans / MultiKMeans).
+"""torchpq_b200 -- H100-native (sm_90a) IVFPQ search path behind torchpq.index.IVFPQIndex.search(), IVFPQ search
+re-ranked on a second PQ code (IVFPQRIndex), exact flat search (FlatIndex), and k-means (clustering.KMeans / MultiKMeans).
 
 Importing this package loads ``libtpq_b200.so``; there is no CPU / PyTorch fallback.
 """
 from . import _lib  # noqa: F401  (raises ImportError when the CUDA library is missing)
 from .index import IVFPQIndex, ScanLayout
 from .flat_index import FlatIndex
+from .ivfpqr_index import IVFPQRIndex
 from . import fn
 from . import clustering
 from .clustering import KMeans, MultiKMeans
 from .patch import patch, unpatch
 
-__all__ = ["IVFPQIndex", "FlatIndex", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "patch", "unpatch"]
+__all__ = ["IVFPQIndex", "IVFPQRIndex", "FlatIndex", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "patch", "unpatch"]

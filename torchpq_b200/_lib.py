@@ -35,7 +35,7 @@ class TpqIndex(C.Structure):
         ("n_blocks", C.c_int64),
         ("codes_scan", C.c_void_p), ("block_valid", C.c_void_p), ("cell_block_start", C.c_void_p),
         ("pq_codebook_t", C.c_void_p), ("pq_norm_t", C.c_void_p),
-        ("part2_scan", C.c_void_p), ("residual", C.c_int32), ("reserved1", C.c_int32),
+        ("part2_scan", C.c_void_p), ("residual", C.c_int32), ("code_size", C.c_int32),
     ]
 
 
@@ -81,6 +81,8 @@ SIGNATURES = {
     "tpq_flat_norms": (_I, [_P, _I64, _I, _I64, _I, _P, _P]),
     "tpq_flat_workspace_bytes": (_SZ, [_I, _I, _I64, _I]),
     "tpq_flat_search": (_I, [_P, _I, _I, _P, _I64, _I64, _P, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
+    "tpq_rerank_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "tpq_rerank": (_I, [_P, _I, _I, _P, _I, _P, _I64, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 

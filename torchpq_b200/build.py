@@ -192,7 +192,8 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
     write = fn.get_write_address(cells, ioa, index._cell_start, index._cell_size, index._cell_capacity, prefix)
     ix = lay.cindex if in_sync else _lib.TpqIndex()
     if not in_sync:
-        ix.n_subvectors, ix.n_cells, ix.capacity = index.code_size, index.n_cells, index.capacity
+        ix.n_subvectors, ix.n_cells, ix.capacity = index.n_subvectors, index.n_cells, index.capacity
+        ix.code_size = index.code_size
         ix.shard_world = 1
     ix.cell_start = index._cell_start.data_ptr()
     check(lib.tpq_store_codes(ptr(codes), ptr(cells), ptr(write), ptr(ids), n, C.byref(ix),

@@ -155,7 +155,8 @@ __global__ void write_address_kernel(const int64_t* __restrict__ cells, const in
 // One thread per (item, 4-code word): storage[g][adr] = codes[4g..4g+3][i] (CellContainer.py:213-239); word 0's thread
 // also does the bookkeeping of CellContainer.add's tail (:354-360).  _cell_size is kept as the cell's high-water mark
 // (atomicMax of slot + 1): without holes that IS old size + count.  If a scan layout is given it receives the same codes,
-// lane-rotated (scan_layout.cuh), and the block's valid bit.
+// lane-rotated (scan_layout.cuh), and the block's valid bit.  A code wider than the scanned one (code_size > M, the
+// re-rank code of IVFPQRIndex) has more word planes; only the first M/4 are scanned and reach the scan layout.
 __global__ void store_codes_kernel(const uint8_t* __restrict__ codes, const int64_t* __restrict__ cells,
                                    const int64_t* __restrict__ write_adr, const int64_t* __restrict__ ids, int64_t n, int M,
                                    int64_t cap, uint32_t* __restrict__ storage, int64_t* __restrict__ address2id,
@@ -179,7 +180,7 @@ __global__ void store_codes_kernel(const uint8_t* __restrict__ codes, const int6
     is_empty[a] = 0;
     atomicMax(cell_size + c, (long long)(pos + 1));
   }
-  if (codes_scan && shard_owns(c, shard_rank, shard_world)) {
+  if (codes_scan && g < M / 4 && shard_owns(c, shard_rank, shard_world)) {
     const int64_t B = (int64_t)cell_block_start[c] + (pos >> 5);
     const int lane = (int)(pos & 31);
     #pragma unroll
@@ -282,9 +283,12 @@ extern "C" int tpq_store_codes(const uint8_t* codes, const int64_t* cells, const
   TPQ_REQUIRE(codes && cells && write_adr && ids && storage && address2id && is_empty && cell_size && ix->cell_start,
               "tpq_store_codes: null pointer");
   const int M = ix->n_subvectors;
+  const int code_size = ix->code_size ? ix->code_size : M;
   TPQ_REQUIRE(M > 0 && M % 4 == 0, "n_subvectors must be a positive multiple of 4, got %d", M);
+  TPQ_REQUIRE(code_size >= M && code_size % 4 == 0, "code_size=%d must be 0 or a multiple of 4 that is >= n_subvectors=%d",
+              ix->code_size, M);
   TPQ_REQUIRE(!codes_scan || (block_valid && ix->cell_block_start && ix->m_pad == scan_m_pad(M)), "tpq_store_codes: incomplete scan layout");
-  dim3 grid((unsigned)((n + 255) / 256), M / 4);
+  dim3 grid((unsigned)((n + 255) / 256), code_size / 4);
   store_codes_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
       codes, cells, write_adr, ids, n, M, ix->capacity, reinterpret_cast<uint32_t*>(storage), address2id, is_empty,
       reinterpret_cast<long long*>(cell_size), ix->cell_start, codes_scan, block_valid, ix->cell_block_start, ix->m_pad,

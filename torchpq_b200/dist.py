@@ -180,6 +180,8 @@ def distribute(index, src: int = 0, group=None, grid=None):
     replicated state (codebooks, per-cell tables, address->id) -- no rank other than ``src`` ever sees the
     reference-layout code store, and ``src`` drops it too unless ``keep_full``.  After the call ``index`` on every
     rank is a shard-only index ready for ``sharded_search``."""
+    if hasattr(index, "n_subvectors_rerank"):
+        raise NotImplementedError("an IVFPQRIndex cannot be distributed: its re-rank pass reads the full _storage")
     world = dist.get_world_size(group)
     rank = dist.get_rank(group)
     shards, groups = grid if grid is not None else (world, 1)

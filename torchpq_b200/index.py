@@ -76,6 +76,7 @@ class ScanLayout:
         ix.cell_size = index._cell_size.data_ptr()
         ix.address2id = index._address2id.data_ptr()
         ix.m_pad, ix.shard_rank, ix.shard_world = self.m_pad, shard_rank, shard_world
+        ix.code_size = getattr(index, "code_size", M)                      # bytes per item in _storage (add writes them all)
         ix.n_blocks = self.n_blocks
         ix.codes_scan = self.codes_scan.data_ptr()
         ix.block_valid = self.block_valid.data_ptr()

@@ -22,6 +22,9 @@ def patch(index):
                  "_cell_size", "_address2id", "vq_codec", "pq_codec"):
         assert hasattr(index, name), f"not an IVFPQIndex-shaped object: missing {name!r}"
     assert index.distance in ("euclidean", "cosine"), "only euclidean and cosine indexes can be searched"
+    if hasattr(index, "n_subvectors_rerank"):
+        raise NotImplementedError("patch() takes IVFPQIndex objects; an IVFPQRIndex needs its re-rank pass: "
+                                  "load its state_dict into torchpq_b200.IVFPQRIndex instead")
     d = index.__dict__
     d["_layout"] = None
     d["_shard"] = (0, 1)
