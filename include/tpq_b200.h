@@ -167,6 +167,18 @@ int tpq_flat_search(const float* x_dn, int d, int nq, const float* base, int64_t
                     const float* norms, int metric, int k, const int64_t* address2id,
                     float* values, int64_t* ids, int64_t* address, void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ row-wise top-k (fn.Topk, fn/Topk.py:43-67)
+ * x [m, n] row-major, contiguous, fp32 or fp16 (dtype TPQ_DTYPE_*) -> the k best entries of every row: values [m, k]
+ * f32 (an fp16 value widened exactly), indices [m, k] i64 (the column).  Order: value descending, then column
+ * ascending; +0 ranks above -0 and every NaN, of either sign, above +inf (returned as a NaN, payload not kept).  A row
+ * with fewer than k entries is padded with (-inf, -1).  1 <= k <= 1024 and n < 2^32 (TPQ_ERR_UNSUPPORTED beyond);
+ * m == 0 returns at once; x may be NULL when n == 0.  ws: at least tpq_topk_workspace_bytes(m, n, k, dtype) bytes (0 bytes, ws may be NULL, when
+ * every row is selected by one CTA or one warp); TPQ_ERR_WORKSPACE when it is smaller. */
+enum { TPQ_DTYPE_F32 = 0, TPQ_DTYPE_F16 = 1 };
+size_t tpq_topk_workspace_bytes(int64_t m, int64_t n, int k, int dtype);
+int tpq_topk(const void* x, int64_t m, int64_t n, int dtype, int k,
+             float* values, int64_t* indices, void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------ re-rank (IVFPQRIndex.search, second pass)
  * candidates [nq, k1] i64: the first pass's addresses (-1 = none), k <= k1 <= 1024.  storage [(M + Mr)/4, capacity, 4]
  * u8 as tpq_index.storage with code_size = M + Mr: bytes 0..M-1 of an item are its first-level code, M..M+Mr-1 its

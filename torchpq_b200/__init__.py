@@ -1,5 +1,6 @@
 """torchpq_b200 -- H100-native (sm_90a) IVFPQ search path behind torchpq.index.IVFPQIndex.search(), IVFPQ search
-re-ranked on a second PQ code (IVFPQRIndex), exact flat search (FlatIndex), and k-means (clustering.KMeans / MultiKMeans).
+re-ranked on a second PQ code (IVFPQRIndex), exact flat search (FlatIndex), row-wise top-k (topk = fn.Topk()), and k-means
+(clustering.KMeans / MultiKMeans).
 
 Importing this package loads ``libtpq_b200.so``; there is no CPU / PyTorch fallback.
 """
@@ -12,4 +13,6 @@ from . import clustering
 from .clustering import KMeans, MultiKMeans
 from .patch import patch, unpatch
 
-__all__ = ["IVFPQIndex", "IVFPQRIndex", "FlatIndex", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "patch", "unpatch"]
+topk = fn.Topk()                     # torchpq.topk (torchpq/__init__.py:22)
+
+__all__ = ["IVFPQIndex", "IVFPQRIndex", "FlatIndex", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "topk", "patch", "unpatch"]

@@ -4,6 +4,7 @@
     precompute_adc       torchpq/codec/PQCodec.py:62-75
     coarse_probe         torchpq/metric.py:74-94 + fn/Topk.py:43-67 + index/IVFPQIndex.py:499-512
     normalize            torchpq/util.py:38-43
+    Topk                 torchpq/fn/Topk.py:43-67 -> kernels/cuda/top1_select.cu, top32_select.cu, topk_select.cu
 Each is one call into the sm_90a library; tensors are passed as raw device pointers.
 """
 from __future__ import annotations
@@ -162,6 +163,39 @@ def merge_topk(keys, address2id):
     check(lib.tpq_merge_topk(ptr(keys), nq, n_parts, k, ptr(address2id), address2id.shape[0],
                              ptr(values), ptr(ids), ptr(address), _lib.current_stream(dev)))
     return values, ids, address
+
+
+class Topk:
+    """fn.Topk (fn/Topk.py:43-67): row-wise top-k of a 2-D CUDA tensor, fp32 or fp16, on one sm_90a select kernel.
+
+    ``__call__(x, k=1, dim=1)`` -> (values [m, k] in x.dtype, indices [m, k] int64).  Order: value descending, then
+    column ascending; +0 ranks above -0 and every NaN, of either sign, above +inf.  Rows shorter than k are padded with
+    (-inf, -1).  k > 1024 raises NotImplementedError (the reference falls back to torch.topk; this package has no
+    torch fallback)."""
+
+    def __call__(self, x, k=1, dim=1):
+        if dim == -1:
+            dim = 1
+        assert dim == 1, "only support last dimention"
+        assert len(x.shape) == 2, "only support 2d tensors"
+        assert x.is_contiguous(), "x is not contiguous"
+        assert k >= 1
+        assert x.device.type == "cuda"
+        assert x.dtype in (torch.float32, torch.float16), f"x must be float32 or float16, got {x.dtype}"
+        k = int(k)
+        if k > 1024:
+            raise NotImplementedError(f"Topk: k={k} > 1024 is not supported")
+        m, n = x.shape
+        dtype = _lib.DTYPE_F32 if x.dtype == torch.float32 else _lib.DTYPE_F16
+        dev = x.device
+        values = torch.empty(m, k, dtype=torch.float32, device=dev)
+        indices = torch.empty(m, k, dtype=torch.int64, device=dev)
+        ws_bytes = lib.tpq_topk_workspace_bytes(m, n, k, dtype)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
+        with torch.cuda.device(dev):
+            check(lib.tpq_topk(ptr(x), m, n, dtype, k, ptr(values), ptr(indices), ptr(ws), ws_bytes,
+                               _lib.current_stream(dev)))
+        return values.to(x.dtype), indices
 
 
 # ------------------------------------------------------------------ build side (CellContainer.add, CellContainer.py:313-367)
