@@ -167,6 +167,30 @@ int tpq_flat_search(const float* x_dn, int d, int nq, const float* base, int64_t
                     const float* norms, int metric, int k, const int64_t* address2id,
                     float* values, int64_t* ids, int64_t* address, void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ IVF search with exact fp32 distances (IVFFlatIndex)
+ * The store is the IVFPQ cell container with fp32 columns: storage [d, capacity] f32 (tpq_store_codes with code_size =
+ * 4 d bytes), is_empty [capacity], cell_start / cell_size [n_cells]; capacity < 2^32.  norms [capacity]: tpq_flat_norms
+ * of every slot (|b|^2 for EUCLIDEAN, |b| + 1e-8 for COSINE), valid for the current store.
+ * cells == NULL: the coarse probe of tpq_ivfpq_search runs inside (x normalised by tpq_normalize_columns for COSINE;
+ *   n_probe <= n_cells, n_probe > 1024 TPQ_ERR_UNSUPPORTED); else cells [nq, n_probe] i64 and n_probe_list [nq] i64 as
+ *   for tpq_ivfpq_search_cells (smart and temperature unused).
+ * Visited: the first probe_count(n_probe_list[q], n_probe) = max(1, min((int)n_probe_list[q], n_probe)) entries, skipping
+ *   cells outside [0, n_cells) and an entry whose cell_start equals the previous entry's; a visited cell's live slots of
+ *   [cell_start, cell_start + cell_size) are scored.  Scores are tpq_flat_search's, bit for bit:
+ *   EUCLIDEAN ((2 x.b) - |x|^2) - |b|^2      COSINE (x / (|x| + 1e-8)).b / (|b| + 1e-8)
+ * -> values [nq, k] f32 descending (-inf padded), ids [nq, k] i64 (address2id[address], -1 padded), address [nq, k] i64
+ *   (nullable, -1 padded).  Order: score descending, then address ascending; independent of the batch and its chunking.
+ *   k > 1024 and metrics other than the two above: TPQ_ERR_UNSUPPORTED.  Arguments are checked before any launch;
+ *   nq == 0 returns at once.  ws: at least tpq_ivfflat_workspace_bytes(d, nq, n_cells, n_probe, k) bytes, which stops
+ *   growing with nq past one chunk of queries (the most whose n_probe * k keys fit 256 MB, at most 16 384). */
+size_t tpq_ivfflat_workspace_bytes(int d, int nq, int n_cells, int n_probe, int k);
+int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                       const float* storage, int64_t capacity, const uint8_t* is_empty,
+                       const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
+                       const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart, float temperature,
+                       int k, const int64_t* address2id, float* values, int64_t* ids, int64_t* address,
+                       void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------ row-wise top-k (fn.Topk, fn/Topk.py:43-67)
  * x [m, n] row-major, contiguous, fp32 or fp16 (dtype TPQ_DTYPE_*) -> the k best entries of every row: values [m, k]
  * f32 (an fp16 value widened exactly), indices [m, k] i64 (the column).  Order: value descending, then column

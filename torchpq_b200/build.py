@@ -97,13 +97,19 @@ def multi_kmeans(data: torch.Tensor, k: int, max_iter: int, tol: float = 1e-4, s
     return fit(data, k, max_iter, tol=tol, n_redo=1, seed=seed, distance=distance)[0]
 
 
-def train(index, x: torch.Tensor, seed: int = 0, vq_iters: int = 15, pq_iters: int = 25):
-    """IVFPQIndex.train: fit the coarse quantizer and the M sub-quantizers on x [d, n]."""
+def train_coarse(index, x: torch.Tensor, seed: int = 0, vq_iters: int = 15):
+    """The coarse half of IVFPQIndex.train: x [d, n] (normalised for cosine) -> (that x, the coarse codebook [d, n_cells]).
+    IVFFlatIndex.train is this alone, so both indexes trained on the same data and seed probe the same cells."""
     assert x.dim() == 2 and x.shape[0] == index.d_vector
     from . import fn
     if index.distance == "cosine":
         x = fn.normalize(x.contiguous())
-    vq = multi_kmeans(x[None].contiguous(), index.n_cells, vq_iters, seed=seed)[0].contiguous()
+    return x, multi_kmeans(x[None].contiguous(), index.n_cells, vq_iters, seed=seed)[0].contiguous()
+
+
+def train(index, x: torch.Tensor, seed: int = 0, vq_iters: int = 15, pq_iters: int = 25):
+    """IVFPQIndex.train: fit the coarse quantizer and the M sub-quantizers on x [d, n]."""
+    x, vq = train_coarse(index, x, seed, vq_iters)
     if getattr(index, "pq_use_residual", False):                       # IVFPQIndex.py:248-256: PQ learns x - vq(x)
         x = x - vq[:, _assign(x[None].contiguous(), vq[None])[0]]
     sub = x.reshape(index.n_subvectors, index.d_subvector, x.shape[1]).contiguous()
@@ -132,7 +138,7 @@ def _expand(index, grow: torch.Tensor):
     shift = torch.cumsum(grow, 0) - grow                           # slots inserted before each cell
     old_cap = index.capacity
     new_cap = old_cap + int(grow.sum().item())
-    storage = torch.zeros(index._storage.shape[0], new_cap, 4, dtype=torch.uint8, device=dev)
+    storage = index._storage.new_zeros((index._storage.shape[0], new_cap, index._storage.shape[2]))   # u8 codes or f32
     a2i = torch.full((new_cap,), -1, dtype=torch.long, device=dev)
     emp = torch.ones(new_cap, dtype=torch.uint8, device=dev)
     check(lib.tpq_expand_move(ptr(index._storage), ptr(index._address2id), ptr(index._is_empty), ptr(index._cell_start),
@@ -147,7 +153,9 @@ def _expand(index, grow: torch.Tensor):
 
 def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, return_address=False):
     """CellContainer.add (CellContainer.py:313-367) on the library's placement kernels (csrc/place.cu): index of
-    appearance, expansion test, write addresses, and one scatter into the reference layout AND the scan layout."""
+    appearance, expansion test, write addresses, and one scatter into the reference layout AND the scan layout.
+    An index without a scan layout (IVFFlatIndex: no ``_layout``, codes = the bytes of its fp32 columns) gets the
+    reference layout only."""
     import ctypes as C
     from . import fn, _lib
     from ._lib import lib, check, ptr
@@ -166,7 +174,7 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
         return (ids, torch.empty(0, dtype=torch.long, device=dev)) if return_address else ids
     codes, cells = codes.contiguous(), cells.contiguous()
     assert int(cells.min().item()) >= 0 and int(cells.max().item()) < index.n_cells, "cell id out of range"
-    lay = index._layout
+    lay = getattr(index, "_layout", None)
     fp = lambda: _fingerprint(index._storage, index._is_empty, index._cell_start, index._cell_size, index._address2id,
                               _codebook_of(index.vq_codec), _codebook_of(index.pq_codec))
     in_sync = lay is not None and lay.fingerprint == fp()
@@ -192,7 +200,8 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
     write = fn.get_write_address(cells, ioa, index._cell_start, index._cell_size, index._cell_capacity, prefix)
     ix = lay.cindex if in_sync else _lib.TpqIndex()
     if not in_sync:
-        ix.n_subvectors, ix.n_cells, ix.capacity = index.n_subvectors, index.n_cells, index.capacity
+        # no scanned code without a scan layout: 4, the smallest n_subvectors tpq_store_codes takes, for a flat store
+        ix.n_subvectors, ix.n_cells, ix.capacity = getattr(index, "n_subvectors", 4), index.n_cells, index.capacity
         ix.code_size = index.code_size
         ix.shard_world = 1
     ix.cell_start = index._cell_start.data_ptr()
@@ -224,3 +233,25 @@ def add(index, x: torch.Tensor, ids=None, return_address=False, chunk: int = 1 <
         cells_l.append(c)
         codes_l.append(q)
     return container_add(index, torch.cat(codes_l, 1), torch.cat(cells_l, 0), ids, return_address)
+
+
+def container_remove(index, ids=None, address=None):
+    """CellContainer.remove (CellContainer.py:369-393) as it is documented to behave (README.md:60-66: "virtually
+    remove vectors ... ignores ids that don't exist"); see IVFPQIndex.remove.  Removed slots become holes (is_empty = 1,
+    address2id = -1); ``_cell_size`` is not decremented."""
+    if ids is not None:
+        address = index.get_address_by_id(ids)
+    elif address is not None:
+        assert address.dtype == torch.int64
+        address = address.to(index._address2id.device)
+    else:
+        raise RuntimeError("Need either ids or address")
+    mask = (address >= 0) & (address < index.capacity)
+    address = address[mask].unique(sorted=True)
+    address = address[index._is_empty[address] == 0]
+    if address.shape[0] == 0:
+        return
+    index._is_empty[address] = 1
+    index._address2id[address] = -1
+    index._has_holes = True
+    index._state_changed()

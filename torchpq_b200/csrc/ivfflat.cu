@@ -1,0 +1,390 @@
+// IVFFlatIndex.search: inverted-file search with exact fp32 distances over a flat store.
+//
+// The store is IVFPQ's cell container with fp32 columns: _storage [d, capacity] (tpq_store_codes with code_size = 4 d
+// bytes), cell c holding slots [cell_start[c], cell_start[c] + cell_capacity[c]) of which [start, start + cell_size) are
+// scanned, holes marked in is_empty.  A query visits the cells of its probe list by the IVFPQ rule (probe_count and
+// probe_visits, scan_layout.cuh) and scores every live vector there with flat.cu's GEMM tile and epilogues, so a score
+// is FlatIndex's bit for bit.
+//
+// Cell-major: the (query, probe entry) pairs are grouped by cell and each cell becomes a small GEMM -- the queries that
+// probe it times its vectors -- so a probed cell is read once per chunk of queries, not once per query.  Per chunk:
+//   1. the chunk's queries are copied to a [d, n] matrix; cells == NULL: the coarse probe of tpq_ivfpq_search on it;
+//   2. ivfflat_pairs_count_kernel: the visited pairs per cell, and each pair's rank in its cell;
+//   3. ivfflat_plan_kernel: each cell's pairs padded to the query tile QT, and the work items (cell, query tile, column
+//      slice), largest slice first;
+//   4. ivfflat_pairs_scatter_kernel + ivfflat_gather_kernel: the pairs' queries as one [d, pad_cap] matrix with zero
+//      columns for the padding, which GemmTile<QT>::run reads unmodified;
+//   5. ivfflat_scan_kernel: per item, GEMM + epilogue + is_empty mask + one WarpTopK per pair over the slice's 128-column
+//      tiles -> keys[j * S + slice][q][:] for the pair (query q, entry j); parts no pair writes stay zero (empty);
+//   6. tpq_merge_topk over the n_probe * S parts of every query -> values, ids, address.
+// The key order is total (score descending, address ascending) and every part is an exact top-k of its columns, so the
+// answer does not depend on QT, S or the chunk.
+#include "gemm_tile.cuh"
+#include "scan_layout.cuh"
+
+extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k, const int64_t* address2id,
+                              int64_t capacity, float* values, int64_t* ids, int64_t* address, void* stream);
+
+namespace tpq {
+
+constexpr float kIvfFlatEps = 1e-8f;            // flat.cu's kFlatEps: metric.cosine_similarity's `norm + 1e-8`
+constexpr int kIvfFlatWarps = 8;
+constexpr size_t kIvfFlatKeyBytes = size_t(256) << 20;   // the chunk's keys [n_probe * S, n, k] stay within 256 MB
+constexpr int kIvfFlatMaxChunk = 16384;         // and a chunk holds at most this many queries
+constexpr int kIvfFlatBuckets = 128;            // classes of the largest-first item order (4 per octave)
+constexpr int kIvfFlatMaxSlices = 128;          // n_probe * S parts per query at most (n_probe permitting)
+
+// Shared memory of one CTA, as flat.cu's: GEMM stages | score tile [QT][128] f32 | lists [QT][kp] | staging [8][kTopkBuf].
+static size_t ivfflat_smem_bytes(int qt, int kp) {
+  const size_t stages = 2 * (size_t)GK * (qt + GB) * 4;
+  return stages + (size_t)qt * GB * 4 + (size_t)qt * kp * 8 + (size_t)kIvfFlatWarps * kTopkBuf * 8;
+}
+
+// The plan, read by the workspace size and the search.  Every size is known before the search, from (d, nq, n_cells,
+// n_probe, k) alone:
+//   chunk0: queries per chunk when S = 1, the most whose keys fit kIvfFlatKeyBytes, at most kIvfFlatMaxChunk;
+//   QT:     16, 32 or 64: the smallest that holds a cell's expected pairs (chunk0 * n_probe / n_cells), halved while the
+//           shared memory exceeds 227 KB (k = 1024 gives 16, as in flat.cu);
+//   S:      column slices per (cell, query tile), enough for two CTAs per SM when the pairs make fewer tiles, with
+//           n_probe * S <= max(n_probe, 128) parts per query;
+//   chunk:  queries per chunk with S slices.
+// Per chunk of n queries: pairs = n * n_probe slots; the padded pair columns pad_cap = pairs + min(n_cells, pairs) *
+// (QT - 1) bound sum over cells of round_up(pairs of the cell, QT), and items = S * pad_cap / QT bounds the work items.
+struct IvfFlatPlan {
+  int qt, kp, S, chunk;
+  int64_t pairs, pad_cap, items;
+  size_t smem;
+  size_t keys, xc, xs, xp, xn, coarse, coarse_bytes, sims, cells, npl, cnt, off, slot, pq, pj, itm, xg, total;
+};
+
+static IvfFlatPlan plan_ivfflat(int d, int nq, int n_cells, int n_probe, int k) {
+  IvfFlatPlan P{};
+  P.kp = list_capacity(k);
+  const size_t per_query = (size_t)n_probe * k * 8;
+  auto chunk_of = [&](int S) {
+    size_t c = kIvfFlatKeyBytes / (per_query * S);
+    c = c < (size_t)kIvfFlatMaxChunk ? c : (size_t)kIvfFlatMaxChunk;
+    return (int)(c < 1 ? 1 : (c > (size_t)nq ? (size_t)nq : c));
+  };
+  const int chunk0 = chunk_of(1);
+  const int64_t per_cell = ((int64_t)chunk0 * n_probe + n_cells - 1) / n_cells;
+  P.qt = 16;
+  while (P.qt < 64 && P.qt < per_cell) P.qt *= 2;
+  while (P.qt > 16 && ivfflat_smem_bytes(P.qt, P.kp) > kSmemLimit) P.qt /= 2;
+  P.smem = ivfflat_smem_bytes(P.qt, P.kp);
+  const int64_t tiles = ((int64_t)chunk0 * n_probe + P.qt - 1) / P.qt;
+  const int64_t want = 2 * (int64_t)device_sm_count();
+  const int smax = n_probe >= kIvfFlatMaxSlices ? 1 : kIvfFlatMaxSlices / n_probe;
+  int64_t S = tiles >= want ? 1 : (want + tiles - 1) / tiles;
+  P.S = (int)(S > smax ? smax : S);
+  P.chunk = chunk_of(P.S);
+  P.pairs = (int64_t)P.chunk * n_probe;
+  P.pad_cap = P.pairs + (P.pairs < n_cells ? P.pairs : n_cells) * (P.qt - 1);
+  P.items = P.S * (P.pad_cap / P.qt);
+  const size_t n = (size_t)P.chunk;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t at = o; o += align_up(bytes, 256); return at; };
+  P.keys = take((size_t)n_probe * P.S * n * k * 8);
+  P.xc = take((size_t)d * n * 4);                      // the chunk's queries
+  P.xs = take((size_t)d * n * 4);                      // cosine: normalize_columns(xc, 1e-8), what the GEMM reads
+  P.xp = take((size_t)d * n * 4);                      // cosine: tpq_normalize_columns(xc), what the probe reads
+  P.xn = take(n * 4);                                  // euclidean: |x|^2
+  P.coarse_bytes = tpq_coarse_workspace_bytes(d, (int)n, n_cells);
+  P.coarse = take(P.coarse_bytes);
+  P.sims = take(n * n_probe * 4);
+  P.cells = take(n * n_probe * 8);
+  P.npl = take(n * 8);
+  P.cnt = take(((size_t)n_cells + 2) * 4);             // pairs per cell, then [n_cells] = items, [n_cells + 1] = columns
+  P.off = take((size_t)n_cells * 4);                   // each cell's first padded pair column
+  P.slot = take((size_t)P.pairs * 4);
+  P.pq = take((size_t)P.pad_cap * 4);                  // chunk-local query of each padded pair column (-1: padding)
+  P.pj = take((size_t)P.pad_cap * 4);                  // probe entry of each padded pair column
+  P.itm = take((size_t)P.items * 16);
+  P.xg = take((size_t)d * P.pad_cap * 4);
+  P.total = o;
+  return P;
+}
+
+// thread per (query, entry) of the chunk: the visited pairs counted per cell; slot = the pair's rank in its cell (-1: none)
+__global__ void ivfflat_pairs_count_kernel(const int64_t* __restrict__ cells, const int64_t* __restrict__ npl, int n,
+                                           int n_probe, int n_cells, const int64_t* __restrict__ cell_start,
+                                           const int64_t* __restrict__ cell_size, int* __restrict__ cell_cnt,
+                                           int* __restrict__ slot) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)n * n_probe) return;
+  const int qi = (int)(t / n_probe), j = (int)(t % n_probe);
+  int pos = -1;
+  int64_t s;
+  if (j < probe_count<false>(npl[qi], n_probe) && probe_visits(cells + (size_t)qi * n_probe, j, n_cells, cell_start, s)) {
+    const int64_t c = cells[t];
+    if (cell_size[c] > 0) pos = atomicAdd(cell_cnt + c, 1);
+  }
+  slot[t] = pos;
+}
+
+// One CTA: off[c] = exclusive prefix of round_up(cnt[c], qt); cnt[n_cells] = items, cnt[n_cells + 1] = padded columns.
+// Items: the ceil(cnt / qt) query tiles x S slices of every cell with pairs, ordered by the slice's column tiles
+// descending in classes of 4 per octave.
+__global__ void __launch_bounds__(1024) ivfflat_plan_kernel(int* __restrict__ cnt, const int64_t* __restrict__ cell_size,
+                                                            int n_cells, int qt, int S, int* __restrict__ off,
+                                                            int4* __restrict__ items) {
+  __shared__ int hist[kIvfFlatBuckets], base[kIvfFlatBuckets], wsum[32], carry;
+  const int tid = threadIdx.x;
+  for (int i = tid; i < kIvfFlatBuckets; i += 1024) hist[i] = 0;
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  auto bucket_of = [&](int c) {
+    const int64_t per = ((cell_size[c] + GB - 1) / GB + S - 1) / S;             // column tiles of the largest slice
+    const uint32_t w = (uint32_t)(per < 1 ? 1 : (per > 0x7fffffff ? 0x7fffffff : per));
+    const int lg = 31 - __clz(w);
+    const int sub = lg >= 2 ? (int)((w >> (lg - 2)) & 3u) : (int)((w << (2 - lg)) & 3u);
+    return kIvfFlatBuckets - 1 - min(kIvfFlatBuckets - 1, 4 * lg + sub);       // more work -> smaller bucket index
+  };
+  for (int c0 = 0; c0 < n_cells; c0 += 1024) {
+    const int c = c0 + tid;
+    const int v = c < n_cells ? cnt[c] : 0;
+    const int tiles = (v + qt - 1) / qt;
+    const int incl = cta_inclusive_scan(tiles * qt, wsum, carry);
+    if (c < n_cells) {
+      off[c] = incl - tiles * qt;
+      if (tiles) atomicAdd(&hist[bucket_of(c)], tiles * S);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int s = 0;
+    for (int b = 0; b < kIvfFlatBuckets; ++b) { base[b] = s; s += hist[b]; }
+    cnt[n_cells] = s;
+    cnt[n_cells + 1] = carry;
+  }
+  __syncthreads();
+  for (int c = tid; c < n_cells; c += 1024) {
+    const int tiles = (cnt[c] + qt - 1) / qt;
+    if (!tiles) continue;
+    const int pos = atomicAdd(&base[bucket_of(c)], tiles * S);
+    for (int i = 0; i < tiles * S; ++i) items[pos + i] = make_int4(c, i / S, i % S, 0);
+  }
+}
+
+__global__ void ivfflat_pairs_scatter_kernel(const int64_t* __restrict__ cells, int n, int n_probe,
+                                             const int* __restrict__ slot, const int* __restrict__ off,
+                                             int* __restrict__ pair_q, int* __restrict__ pair_j) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)n * n_probe) return;
+  const int s = slot[t];
+  if (s < 0) return;
+  const int p = off[cells[t]] + s;
+  pair_q[p] = (int)(t / n_probe);
+  pair_j[p] = (int)(t % n_probe);
+}
+
+// xg[g, p] = x[g, pair_q[p]] for the padded pair columns p < cnt[n_cells + 1]; padding columns are zero
+__global__ void ivfflat_gather_kernel(const float* __restrict__ x, int d, int n, const int* __restrict__ pair_q,
+                                      const int* __restrict__ n_cols, int64_t pad_cap, float* __restrict__ xg) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= *n_cols) return;
+  const int q = pair_q[p];
+  for (int g = blockIdx.y; g < d; g += gridDim.y) xg[(size_t)g * pad_cap + p] = q >= 0 ? x[(size_t)g * n + q] : 0.f;
+}
+
+// One CTA per work item (cell, query tile, slice), 256 threads; the CTAs past the chunk's item count return at once.
+// The slice's columns run in 128-column tiles: GemmTile<QT> over the tile's QT pair columns of xg, flat.cu's epilogue
+// (euclidean ((acc * 2) - |x|^2) - norms[a] with norms = |b|^2; cosine acc / norms[a] with norms = |b| + 1e-8 and x
+// normalised), then per pair row a filter against its k-th key and a WarpTopK that never takes an is_empty slot.
+// Two CTAs per SM, as flat_search_kernel.
+template <int QT, int METRIC>
+__global__ void __launch_bounds__(256, 2)
+ivfflat_scan_kernel(const float* __restrict__ xg, int d, int pad_cap, const int* __restrict__ pair_q,
+                    const int* __restrict__ pair_j, const int4* __restrict__ items, const int* __restrict__ cnt,
+                    int n_cells, const int* __restrict__ off, const float* __restrict__ base, int64_t ld,
+                    const uint8_t* __restrict__ is_empty, const int64_t* __restrict__ cell_start,
+                    const int64_t* __restrict__ cell_size, const float* __restrict__ norms, const float* __restrict__ xn,
+                    int n, int S, int k, int kp, uint64_t* __restrict__ keys_out) {
+  using G = GemmTile<QT>;
+  if ((int)blockIdx.x >= cnt[n_cells]) return;
+  const int4 it = items[blockIdx.x];
+  const int cell = it.x, sl = it.z;
+  const int64_t size = cell_size[cell], start = cell_start[cell];
+  const int64_t T = (size + GB - 1) / GB;
+  const int64_t c_begin = start + T * sl / S * GB;
+  const int64_t c_end = start + (T * (sl + 1) / S * GB < size ? T * (sl + 1) / S * GB : size);
+  if (c_begin >= c_end) return;                        // a slice without columns: its parts stay empty
+  const int p0 = off[cell] + it.y * QT;
+  const int rows = cnt[cell] - it.y * QT < QT ? cnt[cell] - it.y * QT : QT;
+  extern __shared__ __align__(16) uint8_t smem[];
+  auto& stages = *reinterpret_cast<typename G::Stages*>(smem);
+  float (*Sc)[GB] = reinterpret_cast<float (*)[GB]>(smem + sizeof(typename G::Stages));
+  uint64_t* lists = reinterpret_cast<uint64_t*>(smem + sizeof(typename G::Stages) + (size_t)QT * GB * 4);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, tx = tid & 15, ty = tid >> 4;
+  uint64_t* wbuf = lists + (size_t)QT * kp + (size_t)warp * kTopkBuf;
+  float a2[G::MI];
+  #pragma unroll
+  for (int i = 0; i < G::MI; ++i) {
+    const int r = G::row(i, ty);
+    a2[i] = (METRIC == TPQ_METRIC_EUCLIDEAN && r < rows) ? xn[pair_q[p0 + r]] : 0.f;
+  }
+  for (int i = tid; i < QT * kp; i += 256) lists[i] = 0ull;
+  // (the barrier after G::run's first stash orders these stores before the first selection, and each selection
+  //  before the next tile's score stores)
+  for (int64_t c0 = c_begin; c0 < c_end; c0 += GB) {
+    const int cols = (int)(c_end - c0 < GB ? c_end - c0 : GB);
+    float acc[G::MI][8];
+    G::run(xg, pad_cap, p0, base + c0, ld, cols, d, stages, acc);
+    float nc[8];
+    #pragma unroll
+    for (int j = 0; j < 8; ++j) nc[j] = G::col(j, tx) < cols ? norms[c0 + G::col(j, tx)] : 1.f;
+    #pragma unroll
+    for (int i = 0; i < G::MI; ++i) {
+      const int r = G::row(i, ty);
+      float o[8];
+      #pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        if (METRIC == TPQ_METRIC_EUCLIDEAN) o[j] = __fsub_rn(__fsub_rn(__fmul_rn(acc[i][j], 2.f), a2[i]), nc[j]);
+        else o[j] = __fdiv_rn(acc[i][j], nc[j]);
+      }
+      *reinterpret_cast<float4*>(&Sc[r][tx * 4]) = make_float4(o[0], o[1], o[2], o[3]);
+      *reinterpret_cast<float4*>(&Sc[r][64 + tx * 4]) = make_float4(o[4], o[5], o[6], o[7]);
+    }
+    __syncthreads();
+    bool live[4];
+    #pragma unroll
+    for (int u = 0; u < 4; ++u) live[u] = u * 32 + lane < cols && is_empty[c0 + u * 32 + lane] == 0;
+    for (int r = warp; r < rows; r += kIvfFlatWarps) {
+      WarpTopK tk{lists + (size_t)r * kp, wbuf, kp, k, 0};
+      uint64_t thr = tk.kth();
+      #pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const uint64_t key = live[u] ? make_key(Sc[r][u * 32 + lane], (uint32_t)(c0 + u * 32 + lane)) : 0ull;
+        if (tk.push(live[u] && key > thr, key, lane)) thr = tk.kth();
+      }
+      tk.flush(lane);
+    }
+  }
+  __syncthreads();                                     // the lists were last written by their own warps
+  for (int r = warp; r < rows; r += kIvfFlatWarps) {
+    const int p = p0 + r;
+    uint64_t* dst = keys_out + (((size_t)pair_j[p] * S + sl) * n + pair_q[p]) * k;
+    for (int i = lane; i < k; i += 32) dst[i] = lists[(size_t)r * kp + i];
+  }
+}
+
+}  // namespace tpq
+
+using namespace tpq;
+
+extern "C" size_t tpq_ivfflat_workspace_bytes(int d, int nq, int n_cells, int n_probe, int k) {
+  if (d <= 0 || nq <= 0 || n_cells <= 0 || n_probe <= 0 || k <= 0 || k > 1024) return 0;
+  return plan_ivfflat(d, nq, n_cells, n_probe, k).total;
+}
+
+template <int QT>
+static int launch_ivfflat_scan(int metric, const IvfFlatPlan& P, const float* xg, int d, const int* pair_q,
+                               const int* pair_j, const int4* items, const int* cnt, int n_cells, const int* off,
+                               const float* storage, int64_t capacity, const uint8_t* is_empty,
+                               const int64_t* cell_start, const int64_t* cell_size, const float* norms, const float* xn,
+                               int n, int k, uint64_t* keys, cudaStream_t st) {
+  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? ivfflat_scan_kernel<QT, TPQ_METRIC_EUCLIDEAN>
+                                             : ivfflat_scan_kernel<QT, TPQ_METRIC_COSINE>;
+  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
+  kern<<<(unsigned)P.items, 256, P.smem, st>>>(xg, d, (int)P.pad_cap, pair_q, pair_j, items, cnt, n_cells, off, storage,
+                                               capacity, is_empty, cell_start, cell_size, norms, xn, n, P.S, k, P.kp, keys);
+  TPQ_LAUNCH_CHECK("ivfflat_scan_kernel");
+  return TPQ_OK;
+}
+
+extern "C" int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                                  const float* storage, int64_t capacity, const uint8_t* is_empty,
+                                  const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
+                                  const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart,
+                                  float temperature, int k, const int64_t* address2id, float* values, int64_t* ids,
+                                  int64_t* address, void* ws, size_t ws_bytes, void* stream) {
+  TPQ_REQUIRE(k > 0, "k must be in (0, 1024], got %d", k);
+  if (k > 1024) { set_error("k=%d > 1024 is not supported", k); return TPQ_ERR_UNSUPPORTED; }
+  if (metric != TPQ_METRIC_EUCLIDEAN && metric != TPQ_METRIC_COSINE) {
+    set_error("tpq_ivfflat_search: unsupported metric %d (euclidean and cosine only)", metric);
+    return TPQ_ERR_UNSUPPORTED;
+  }
+  TPQ_REQUIRE(d > 0 && nq >= 0 && n_cells > 0 && n_probe >= 1 && capacity >= 0,
+              "tpq_ivfflat_search: bad sizes d=%d nq=%d n_cells=%d n_probe=%d capacity=%lld", d, nq, n_cells, n_probe,
+              (long long)capacity);
+  TPQ_REQUIRE(capacity < (int64_t(1) << 32), "tpq_ivfflat_search: capacity=%lld exceeds the 32-bit address of a key",
+              (long long)capacity);
+  TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "tpq_ivfflat_search: cells and n_probe_list go together");
+  if (!cells) {
+    TPQ_REQUIRE(n_probe <= n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, n_cells);
+    if (n_probe > 1024) { set_error("n_probe=%d > 1024 is not supported", n_probe); return TPQ_ERR_UNSUPPORTED; }
+  }
+  TPQ_REQUIRE(values && ids, "tpq_ivfflat_search: null output");
+  if (nq == 0) return TPQ_OK;
+  TPQ_REQUIRE(x_dn && cell_start && cell_size && (cells || vq_codebook), "tpq_ivfflat_search: null query or cell table");
+  TPQ_REQUIRE(capacity == 0 || (storage && is_empty && norms && address2id), "tpq_ivfflat_search: null store");
+  const IvfFlatPlan P = plan_ivfflat(d, nq, n_cells, n_probe, k);
+  if (!ws || ws_bytes < P.total) {
+    set_error("tpq_ivfflat_search: workspace too small (%zu < %zu)", ws_bytes, P.total);
+    return TPQ_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  uint64_t* keys = reinterpret_cast<uint64_t*>(w + P.keys);
+  float *xc = reinterpret_cast<float*>(w + P.xc), *xs = reinterpret_cast<float*>(w + P.xs);
+  float *xp = reinterpret_cast<float*>(w + P.xp), *xn = reinterpret_cast<float*>(w + P.xn);
+  int *cnt = reinterpret_cast<int*>(w + P.cnt), *off = reinterpret_cast<int*>(w + P.off);
+  int *slot = reinterpret_cast<int*>(w + P.slot), *pair_q = reinterpret_cast<int*>(w + P.pq);
+  int* pair_j = reinterpret_cast<int*>(w + P.pj);
+  int4* items = reinterpret_cast<int4*>(w + P.itm);
+  float* xg = reinterpret_cast<float*>(w + P.xg);
+  // capacity == 0: every key is empty and the id table is never read, so any non-null pointer will do
+  const int64_t* a2i = capacity ? address2id : reinterpret_cast<const int64_t*>(keys);
+  for (int q0 = 0; q0 < nq; q0 += P.chunk) {
+    const int n = nq - q0 < P.chunk ? nq - q0 : P.chunk;
+    TPQ_CUDA(cudaMemcpy2DAsync(xc, (size_t)n * 4, x_dn + q0, (size_t)nq * 4, (size_t)n * 4, d, cudaMemcpyDeviceToDevice, st));
+    const int64_t *cq = cells ? cells + (size_t)q0 * n_probe : nullptr, *npl = cells ? n_probe_list + q0 : nullptr;
+    if (!cells) {                                      // tpq_ivfpq_search's coarse stage, on the chunk
+      const float* xprobe = xc;
+      if (metric == TPQ_METRIC_COSINE) {
+        if (int rc = tpq_normalize_columns(xc, d, n, xp, stream)) return rc;
+        xprobe = xp;
+      }
+      int64_t *cw = reinterpret_cast<int64_t*>(w + P.cells), *nw = reinterpret_cast<int64_t*>(w + P.npl);
+      if (int rc = tpq_coarse_probe(xprobe, vq_codebook, d, n, n_cells, n_probe, smart, temperature,
+                                    reinterpret_cast<float*>(w + P.sims), cw, nw, w + P.coarse, P.coarse_bytes, stream))
+        return rc;
+      cq = cw; npl = nw;
+    }
+    const float* xq = xc;
+    if (metric == TPQ_METRIC_EUCLIDEAN) {
+      if (int rc = col_sqnorms(xc, d, n, n, xn, st)) return rc;
+    } else {
+      if (int rc = normalize_columns(xc, d, n, kIvfFlatEps, xs, st)) return rc;
+      xq = xs;
+    }
+    const int64_t nt = (int64_t)n * n_probe;
+    const unsigned pgrid = (unsigned)((nt + 255) / 256);
+    TPQ_CUDA(cudaMemsetAsync(cnt, 0, ((size_t)n_cells + 2) * 4, st));
+    TPQ_CUDA(cudaMemsetAsync(pair_q, 0xFF, (size_t)P.pad_cap * 4, st));
+    TPQ_CUDA(cudaMemsetAsync(keys, 0, (size_t)n_probe * P.S * n * k * 8, st));
+    ivfflat_pairs_count_kernel<<<pgrid, 256, 0, st>>>(cq, npl, n, n_probe, n_cells, cell_start, cell_size, cnt, slot);
+    TPQ_LAUNCH_CHECK("ivfflat_pairs_count_kernel");
+    ivfflat_plan_kernel<<<1, 1024, 0, st>>>(cnt, cell_size, n_cells, P.qt, P.S, off, items);
+    TPQ_LAUNCH_CHECK("ivfflat_plan_kernel");
+    ivfflat_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(cq, n, n_probe, slot, off, pair_q, pair_j);
+    TPQ_LAUNCH_CHECK("ivfflat_pairs_scatter_kernel");
+    const dim3 ggrid((unsigned)((P.pad_cap + 255) / 256), (unsigned)(d < 64 ? d : 64));
+    ivfflat_gather_kernel<<<ggrid, 256, 0, st>>>(xq, d, n, pair_q, cnt + n_cells + 1, P.pad_cap, xg);
+    TPQ_LAUNCH_CHECK("ivfflat_gather_kernel");
+    int rc;
+    switch (P.qt) {
+      case 16: rc = launch_ivfflat_scan<16>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage, capacity,
+                                            is_empty, cell_start, cell_size, norms, xn, n, k, keys, st); break;
+      case 32: rc = launch_ivfflat_scan<32>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage, capacity,
+                                            is_empty, cell_start, cell_size, norms, xn, n, k, keys, st); break;
+      default: rc = launch_ivfflat_scan<64>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage, capacity,
+                                            is_empty, cell_start, cell_size, norms, xn, n, k, keys, st); break;
+    }
+    if (rc) return rc;
+    if (int rc2 = tpq_merge_topk(keys, n, n_probe * P.S, k, a2i, capacity, values + (size_t)q0 * k,
+                                 ids + (size_t)q0 * k, address ? address + (size_t)q0 * k : nullptr, stream))
+      return rc2;
+  }
+  return TPQ_OK;
+}

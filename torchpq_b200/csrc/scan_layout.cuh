@@ -61,6 +61,22 @@ __device__ __forceinline__ int probe_count(int64_t n_probe_list_q, int n_probe) 
   return RES ? max(0, min(P, n_probe)) : max(1, min(P, n_probe));
 }
 
+// Which of a query's first P entries are visited, for every probe-list scan (IVFPQ's scan layout and IVFFlat's flat
+// store alike): entry j is skipped when its cell is outside [0, n_cells) (caller-supplied lists are not trusted) or when
+// its cell_start equals that of entry j - 1 (a cell listed twice in a row is scanned once; twice apart, twice).  A visited
+// entry scans its cell's live extent [s, s + cell_size), nothing for an empty cell.  s: the cell's start, -1 outside.
+__device__ __forceinline__ bool probe_visits(const int64_t* cq, int j, int n_cells, const int64_t* cell_start, int64_t& s) {
+  const int64_t c = cq[j];
+  const bool ok = c >= 0 && c < n_cells;
+  s = ok ? cell_start[c] : -1;
+  bool skip = !ok;
+  if (ok && j > 0) {
+    const int64_t cp = cq[j - 1];
+    skip = cp >= 0 && cp < n_cells && s == cell_start[cp];
+  }
+  return !skip;
+}
+
 __host__ __device__ constexpr int64_t scan_blocks(int64_t n) { return n > 0 ? (n + 31) >> 5 : 0; }
 // Blocks a scan reads of a cell whose layout holds blocks [b0, b1): the layout has a block for every slot of the cell's
 // capacity (none for another shard's cell), the live extent is cell_size.
@@ -77,16 +93,12 @@ __device__ __forceinline__ ProbeEntry probe_entry(const int64_t* cq, int j, int 
   ProbeEntry e;
   const int64_t c = cq[j];
   const bool ok = c >= 0 && c < n_cells;
-  const int64_t s = ok ? cell_start[c] : -1;
-  bool skip = !ok;
-  if (ok && j > 0) {
-    const int64_t cp = cq[j - 1];
-    skip = cp >= 0 && cp < n_cells && s == cell_start[cp];
-  }
+  int64_t s;
+  const bool visit = probe_visits(cq, j, n_cells, cell_start, s);
   e.cell = ok ? c : 0;
   e.blk0 = ok ? cell_block_start[c] : 0;
   e.addr0 = (uint32_t)s;
-  e.nb = skip ? 0 : cell_blocks(e.blk0, cell_block_start[c + 1], cell_size[c]);
+  e.nb = visit ? cell_blocks(e.blk0, cell_block_start[c + 1], cell_size[c]) : 0;
   return e;
 }
 

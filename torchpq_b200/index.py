@@ -342,22 +342,8 @@ class IVFPQIndex(IdContainer):
         `add` into the cell fills first.  `_cell_size` is deliberately NOT decremented: search scans
         [cell_start, cell_start + cell_size) (ivfpq_topk.cu:852-853), so shrinking it -- as the reference's dead code
         would -- hides live vectors at the tail of the cell."""
-        if ids is not None:
-            address = self.get_address_by_id(ids)
-        elif address is not None:
-            assert address.dtype == torch.int64
-            address = address.to(self._address2id.device)
-        else:
-            raise RuntimeError("Need either ids or address")
-        mask = (address >= 0) & (address < self.capacity)
-        address = address[mask].unique(sorted=True)
-        address = address[self._is_empty[address] == 0]
-        if address.shape[0] == 0:
-            return
-        self._is_empty[address] = 1
-        self._address2id[address] = -1
-        self._has_holes = True
-        self._state_changed()
+        from . import build
+        build.container_remove(self, ids, address)
 
     def encode(self, x):
         """IVFPQIndex.encode (IVFPQIndex.py:262-287): x [d_vector, n] -> PQ codes [n_subvectors, n] uint8
