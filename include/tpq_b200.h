@@ -191,6 +191,32 @@ int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codeboo
                        int k, const int64_t* address2id, float* values, int64_t* ids, int64_t* address,
                        void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ scalar quantization (SQCodec, IVFSQIndex)
+ * tpq_sq_encode: x_dn [d, n] f32 -> out [d, n]: u8 for bits 8, fp16 for bits 16, f32 (a copy) for bits 32.
+ * tpq_sq_decode: codes [d, n] in the same types -> out_dn [d, n] f32.  lower / range [d] f32 (bits 8 only, NULL
+ *   otherwise allowed): the codec's trained bounds, range = upper - lower + 1e-8.  Bit for bit the reference's torch ops:
+ *   encode 8  clamp(rint(((x - lower) / range) * 256), 0, 255)    (each op rounded, rint half to even; NaN -> 0)
+ *   decode 8  ((code / 256) * range) + lower                       (two roundings, no fma)
+ *   16 bits   __float2half_rn / __half2float (beyond +-65504: +-inf)
+ *   bits other than 8, 16, 32: TPQ_ERR_UNSUPPORTED.  n == 0 returns at once.  Inputs are never written.
+ * tpq_ivfsq_search: tpq_ivfflat_search over an SQ-coded store, scored on the decoded vectors: storage is
+ *   [code_size / 4, capacity, 4] u8 as tpq_index.storage (word planes, row stride capacity words) with code_size = d
+ *   (bits 8, d % 4 == 0) or 2 d (bits 16, d % 2 == 0); byte j of an item is the code of dimension j (bits 8), bytes
+ *   2 j, 2 j + 1 the fp16 code of dimension j (bits 16).  lower / range: as above, 16-byte aligned, read for bits 8.
+ *   norms: tpq_flat_norms of the decoded store.  Values, ids and addresses are tpq_ivfflat_search's on the decoded
+ *   store [d, capacity] f32, bit for bit; the workspace is tpq_ivfflat_workspace_bytes's.  bits other than 8 and 16:
+ *   TPQ_ERR_UNSUPPORTED; every other argument is checked as by tpq_ivfflat_search, before any launch. */
+int tpq_sq_encode(const float* x_dn, int d, int64_t n, int bits, const float* lower, const float* range, void* out,
+                  void* stream);
+int tpq_sq_decode(const void* codes, int d, int64_t n, int bits, const float* lower, const float* range, float* out_dn,
+                  void* stream);
+int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                     const uint8_t* storage, int bits, const float* lower, const float* range, int64_t capacity,
+                     const uint8_t* is_empty, const int64_t* cell_start, const int64_t* cell_size, const float* norms,
+                     int metric, const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart,
+                     float temperature, int k, const int64_t* address2id, float* values, int64_t* ids,
+                     int64_t* address, void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------ row-wise top-k (fn.Topk, fn/Topk.py:43-67)
  * x [m, n] row-major, contiguous, fp32 or fp16 (dtype TPQ_DTYPE_*) -> the k best entries of every row: values [m, k]
  * f32 (an fp16 value widened exactly), indices [m, k] i64 (the column).  Order: value descending, then column

@@ -1,6 +1,6 @@
 """torchpq_b200 -- H100-native (sm_90a) IVFPQ search path behind torchpq.index.IVFPQIndex.search(), IVFPQ search
 re-ranked on a second PQ code (IVFPQRIndex), exact flat search (FlatIndex), inverted-file search with exact distances
-(IVFFlatIndex), row-wise top-k (topk = fn.Topk()), and k-means
+(IVFFlatIndex), inverted-file search over scalar-quantized vectors (IVFSQIndex, codec.SQCodec), row-wise top-k (topk = fn.Topk()), and k-means
 (clustering.KMeans / MultiKMeans).
 
 Importing this package loads ``libtpq_b200.so``; there is no CPU / PyTorch fallback.
@@ -10,6 +10,8 @@ from .index import IVFPQIndex, ScanLayout
 from .flat_index import FlatIndex
 from .ivfpqr_index import IVFPQRIndex
 from .ivfflat_index import IVFFlatIndex
+from .ivfsq_index import IVFSQIndex
+from . import codec
 from . import fn
 from . import clustering
 from .clustering import KMeans, MultiKMeans
@@ -17,4 +19,4 @@ from .patch import patch, unpatch
 
 topk = fn.Topk()                     # torchpq.topk (torchpq/__init__.py:22)
 
-__all__ = ["IVFPQIndex", "IVFPQRIndex", "IVFFlatIndex", "FlatIndex", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "topk", "patch", "unpatch"]
+__all__ = ["IVFPQIndex", "IVFPQRIndex", "IVFFlatIndex", "IVFSQIndex", "FlatIndex", "codec", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "topk", "patch", "unpatch"]

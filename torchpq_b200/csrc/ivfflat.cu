@@ -19,6 +19,9 @@
 //   6. tpq_merge_topk over the n_probe * S parts of every query -> values, ids, address.
 // The key order is total (score descending, address ascending) and every part is an exact top-k of its columns, so the
 // answer does not depend on QT, S or the chunk.
+// IVFSQIndex.search (tpq_ivfsq_search) is the same search over an SQCodec-coded store (word planes of 8-bit codes or
+// fp16): its scan instances read the codes through gemm_tile.cuh's BLoadSQ8 / BLoadSQ16, which decode them as the tile
+// stages them, so its scores are this search's over the decoded store, bit for bit.
 #include "gemm_tile.cuh"
 #include "scan_layout.cuh"
 
@@ -191,16 +194,19 @@ __global__ void ivfflat_gather_kernel(const float* __restrict__ x, int d, int n,
 // The slice's columns run in 128-column tiles: GemmTile<QT> over the tile's QT pair columns of xg, flat.cu's epilogue
 // (euclidean ((acc * 2) - |x|^2) - norms[a] with norms = |b|^2; cosine acc / norms[a] with norms = |b| + 1e-8 and x
 // normalised), then per pair row a filter against its k-th key and a WarpTopK that never takes an is_empty slot.
-// Two CTAs per SM, as flat_search_kernel.
-template <int QT, int METRIC>
+// Two CTAs per SM, as flat_search_kernel.  BL is the store's B loader (gemm_tile.cuh): BLoadF32 for IVFFlatIndex's fp32
+// columns, BLoadSQ8 / BLoadSQ16 for IVFSQIndex's code words, decoded as the tile stages them, so that an SQ store scores
+// exactly as its decoded fp32 image would.  base [*, ld] is the store, `extra` the loader's own pointers (SQ8: lower,
+// range), last so that the fp32 instances keep IVFFlatIndex's parameter list.
+template <int QT, int METRIC, class BL, class... Extra>
 __global__ void __launch_bounds__(256, 2)
 ivfflat_scan_kernel(const float* __restrict__ xg, int d, int pad_cap, const int* __restrict__ pair_q,
                     const int* __restrict__ pair_j, const int4* __restrict__ items, const int* __restrict__ cnt,
-                    int n_cells, const int* __restrict__ off, const float* __restrict__ base, int64_t ld,
+                    int n_cells, const int* __restrict__ off, const typename BL::T* __restrict__ base, int64_t ld,
                     const uint8_t* __restrict__ is_empty, const int64_t* __restrict__ cell_start,
                     const int64_t* __restrict__ cell_size, const float* __restrict__ norms, const float* __restrict__ xn,
-                    int n, int S, int k, int kp, uint64_t* __restrict__ keys_out) {
-  using G = GemmTile<QT>;
+                    int n, int S, int k, int kp, uint64_t* __restrict__ keys_out, Extra... extra) {
+  using G = GemmTile<QT, BL>;
   if ((int)blockIdx.x >= cnt[n_cells]) return;
   const int4 it = items[blockIdx.x];
   const int cell = it.x, sl = it.z;
@@ -229,7 +235,7 @@ ivfflat_scan_kernel(const float* __restrict__ xg, int d, int pad_cap, const int*
   for (int64_t c0 = c_begin; c0 < c_end; c0 += GB) {
     const int cols = (int)(c_end - c0 < GB ? c_end - c0 : GB);
     float acc[G::MI][8];
-    G::run(xg, pad_cap, p0, base + c0, ld, cols, d, stages, acc);
+    G::run(xg, pad_cap, p0, BL{base + c0, ld, extra...}, cols, d, stages, acc);
     float nc[8];
     #pragma unroll
     for (int j = 0; j < 8; ++j) nc[j] = G::col(j, tx) < cols ? norms[c0 + G::col(j, tx)] : 1.f;
@@ -277,50 +283,54 @@ extern "C" size_t tpq_ivfflat_workspace_bytes(int d, int nq, int n_cells, int n_
   return plan_ivfflat(d, nq, n_cells, n_probe, k).total;
 }
 
-template <int QT>
+template <int QT, class BL, class... Extra>
 static int launch_ivfflat_scan(int metric, const IvfFlatPlan& P, const float* xg, int d, const int* pair_q,
                                const int* pair_j, const int4* items, const int* cnt, int n_cells, const int* off,
-                               const float* storage, int64_t capacity, const uint8_t* is_empty,
+                               const typename BL::T* storage, int64_t capacity, const uint8_t* is_empty,
                                const int64_t* cell_start, const int64_t* cell_size, const float* norms, const float* xn,
-                               int n, int k, uint64_t* keys, cudaStream_t st) {
-  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? ivfflat_scan_kernel<QT, TPQ_METRIC_EUCLIDEAN>
-                                             : ivfflat_scan_kernel<QT, TPQ_METRIC_COSINE>;
+                               int n, int k, uint64_t* keys, cudaStream_t st, Extra... extra) {
+  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? ivfflat_scan_kernel<QT, TPQ_METRIC_EUCLIDEAN, BL, Extra...>
+                                             : ivfflat_scan_kernel<QT, TPQ_METRIC_COSINE, BL, Extra...>;
   TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
   kern<<<(unsigned)P.items, 256, P.smem, st>>>(xg, d, (int)P.pad_cap, pair_q, pair_j, items, cnt, n_cells, off, storage,
-                                               capacity, is_empty, cell_start, cell_size, norms, xn, n, P.S, k, P.kp, keys);
+                                               capacity, is_empty, cell_start, cell_size, norms, xn, n, P.S, k, P.kp,
+                                               keys, extra...);
   TPQ_LAUNCH_CHECK("ivfflat_scan_kernel");
   return TPQ_OK;
 }
 
-extern "C" int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
-                                  const float* storage, int64_t capacity, const uint8_t* is_empty,
-                                  const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
-                                  const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart,
-                                  float temperature, int k, const int64_t* address2id, float* values, int64_t* ids,
-                                  int64_t* address, void* ws, size_t ws_bytes, void* stream) {
+// The body of tpq_ivfflat_search and tpq_ivfsq_search: `name` prefixes the messages, BL reads the store (storage
+// [*, capacity] words) and `extra` are its own pointers, checked by the caller.
+template <class BL, class... Extra>
+static int ivf_search(const char* name, const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                      const typename BL::T* storage, int64_t capacity, const uint8_t* is_empty,
+                      const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
+                      const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart, float temperature,
+                      int k, const int64_t* address2id, float* values, int64_t* ids, int64_t* address, void* ws,
+                      size_t ws_bytes, void* stream, Extra... extra) {
   TPQ_REQUIRE(k > 0, "k must be in (0, 1024], got %d", k);
   if (k > 1024) { set_error("k=%d > 1024 is not supported", k); return TPQ_ERR_UNSUPPORTED; }
   if (metric != TPQ_METRIC_EUCLIDEAN && metric != TPQ_METRIC_COSINE) {
-    set_error("tpq_ivfflat_search: unsupported metric %d (euclidean and cosine only)", metric);
+    set_error("%s: unsupported metric %d (euclidean and cosine only)", name, metric);
     return TPQ_ERR_UNSUPPORTED;
   }
   TPQ_REQUIRE(d > 0 && nq >= 0 && n_cells > 0 && n_probe >= 1 && capacity >= 0,
-              "tpq_ivfflat_search: bad sizes d=%d nq=%d n_cells=%d n_probe=%d capacity=%lld", d, nq, n_cells, n_probe,
+              "%s: bad sizes d=%d nq=%d n_cells=%d n_probe=%d capacity=%lld", name, d, nq, n_cells, n_probe,
               (long long)capacity);
-  TPQ_REQUIRE(capacity < (int64_t(1) << 32), "tpq_ivfflat_search: capacity=%lld exceeds the 32-bit address of a key",
+  TPQ_REQUIRE(capacity < (int64_t(1) << 32), "%s: capacity=%lld exceeds the 32-bit address of a key", name,
               (long long)capacity);
-  TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "tpq_ivfflat_search: cells and n_probe_list go together");
+  TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "%s: cells and n_probe_list go together", name);
   if (!cells) {
     TPQ_REQUIRE(n_probe <= n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, n_cells);
     if (n_probe > 1024) { set_error("n_probe=%d > 1024 is not supported", n_probe); return TPQ_ERR_UNSUPPORTED; }
   }
-  TPQ_REQUIRE(values && ids, "tpq_ivfflat_search: null output");
+  TPQ_REQUIRE(values && ids, "%s: null output", name);
   if (nq == 0) return TPQ_OK;
-  TPQ_REQUIRE(x_dn && cell_start && cell_size && (cells || vq_codebook), "tpq_ivfflat_search: null query or cell table");
-  TPQ_REQUIRE(capacity == 0 || (storage && is_empty && norms && address2id), "tpq_ivfflat_search: null store");
+  TPQ_REQUIRE(x_dn && cell_start && cell_size && (cells || vq_codebook), "%s: null query or cell table", name);
+  TPQ_REQUIRE(capacity == 0 || (storage && is_empty && norms && address2id), "%s: null store", name);
   const IvfFlatPlan P = plan_ivfflat(d, nq, n_cells, n_probe, k);
   if (!ws || ws_bytes < P.total) {
-    set_error("tpq_ivfflat_search: workspace too small (%zu < %zu)", ws_bytes, P.total);
+    set_error("%s: workspace too small (%zu < %zu)", name, ws_bytes, P.total);
     return TPQ_ERR_WORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
@@ -374,12 +384,15 @@ extern "C" int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float*
     TPQ_LAUNCH_CHECK("ivfflat_gather_kernel");
     int rc;
     switch (P.qt) {
-      case 16: rc = launch_ivfflat_scan<16>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage, capacity,
-                                            is_empty, cell_start, cell_size, norms, xn, n, k, keys, st); break;
-      case 32: rc = launch_ivfflat_scan<32>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage, capacity,
-                                            is_empty, cell_start, cell_size, norms, xn, n, k, keys, st); break;
-      default: rc = launch_ivfflat_scan<64>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage, capacity,
-                                            is_empty, cell_start, cell_size, norms, xn, n, k, keys, st); break;
+      case 16: rc = launch_ivfflat_scan<16, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
+                                                capacity, is_empty, cell_start, cell_size, norms, xn, n, k, keys, st,
+                                                extra...); break;
+      case 32: rc = launch_ivfflat_scan<32, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
+                                                capacity, is_empty, cell_start, cell_size, norms, xn, n, k, keys, st,
+                                                extra...); break;
+      default: rc = launch_ivfflat_scan<64, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
+                                                capacity, is_empty, cell_start, cell_size, norms, xn, n, k, keys, st,
+                                                extra...); break;
     }
     if (rc) return rc;
     if (int rc2 = tpq_merge_topk(keys, n, n_probe * P.S, k, a2i, capacity, values + (size_t)q0 * k,
@@ -387,4 +400,41 @@ extern "C" int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float*
       return rc2;
   }
   return TPQ_OK;
+}
+
+extern "C" int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                                  const float* storage, int64_t capacity, const uint8_t* is_empty,
+                                  const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
+                                  const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart,
+                                  float temperature, int k, const int64_t* address2id, float* values, int64_t* ids,
+                                  int64_t* address, void* ws, size_t ws_bytes, void* stream) {
+  return ivf_search<BLoadF32>("tpq_ivfflat_search", x_dn, d, nq, vq_codebook, n_cells, storage, capacity, is_empty,
+                              cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart, temperature,
+                              k, address2id, values, ids, address, ws, ws_bytes, stream);
+}
+
+extern "C" int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                                const uint8_t* storage, int bits, const float* lower, const float* range,
+                                int64_t capacity, const uint8_t* is_empty, const int64_t* cell_start,
+                                const int64_t* cell_size, const float* norms, int metric, const int64_t* cells,
+                                const int64_t* n_probe_list, int n_probe, int smart, float temperature, int k,
+                                const int64_t* address2id, float* values, int64_t* ids, int64_t* address, void* ws,
+                                size_t ws_bytes, void* stream) {
+  if (bits != 8 && bits != 16) {
+    set_error("tpq_ivfsq_search: bits=%d is not supported (8 and 16 only)", bits);
+    return TPQ_ERR_UNSUPPORTED;
+  }
+  TPQ_REQUIRE(d > 0 && d % (bits == 8 ? 4 : 2) == 0, "tpq_ivfsq_search: d=%d must be a positive multiple of %d for %d bits",
+              d, bits == 8 ? 4 : 2, bits);
+  const uint32_t* words = reinterpret_cast<const uint32_t*>(storage);
+  if (bits == 16)
+    return ivf_search<BLoadSQ16>("tpq_ivfsq_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
+                                 cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
+                                 temperature, k, address2id, values, ids, address, ws, ws_bytes, stream);
+  TPQ_REQUIRE(lower && range, "tpq_ivfsq_search: null lower or range (8 bits)");
+  TPQ_REQUIRE((reinterpret_cast<uintptr_t>(lower) | reinterpret_cast<uintptr_t>(range)) % 16 == 0,
+              "tpq_ivfsq_search: lower and range must be 16-byte aligned");
+  return ivf_search<BLoadSQ8>("tpq_ivfsq_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
+                              cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart, temperature,
+                              k, address2id, values, ids, address, ws, ws_bytes, stream, lower, range);
 }

@@ -46,7 +46,7 @@ class IVFFlatIndex(IdContainer):
         cap = n_cells * initial_size
         self.register_buffer("_address2id", -torch.ones(cap, dtype=torch.long, device=dev))
         self.register_buffer("_id2address", None)
-        self.register_buffer("_storage", torch.zeros(d_vector, cap, 1, dtype=torch.float32, device=dev))
+        self.register_buffer("_storage", self._empty_store(cap, dev))
         self.register_buffer("_cell_start", torch.arange(n_cells, device=dev) * initial_size)
         self.register_buffer("_cell_size", torch.zeros(n_cells, dtype=torch.long, device=dev))
         self.register_buffer("_cell_capacity", torch.zeros(n_cells, dtype=torch.long, device=dev) + initial_size)
@@ -62,10 +62,15 @@ class IVFFlatIndex(IdContainer):
         # dropped explicitly on every change of the store, not only when its fingerprint moves
         self._norms = None
 
+    def _empty_store(self, cap, dev):
+        """A zero store of `cap` slots: fp32 [d, cap, 1]."""
+        return torch.zeros(self.d_vector, cap, 1, dtype=torch.float32, device=dev)
+
     def load_state_dict(self, state_dict, strict=True):
         """As IVFPQIndex.load_state_dict: the buffers, then ``_max_id`` re-derived and holes assumed."""
         super().load_state_dict(state_dict, strict)
-        assert self._storage.dtype == torch.float32 and self._storage.shape == (self.d_vector, self.capacity, 1)
+        want = self._empty_store(0, "meta")
+        assert self._storage.dtype == want.dtype and self._storage.shape == (want.shape[0], self.capacity, want.shape[2])
         self._has_holes = True
         self._refresh_max_id()
 
@@ -145,13 +150,18 @@ class IVFFlatIndex(IdContainer):
         ws_bytes = lib.tpq_ivfflat_workspace_bytes(self.d_vector, nq, self.n_cells, n_probe, k)
         ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
         vq = self.vq_codec.kmeans.centroids if cells is None else None
-        check(lib.tpq_ivfflat_search(ptr(x), self.d_vector, nq, ptr(vq), self.n_cells, ptr(self._storage), self.capacity,
-                                     ptr(self._is_empty), ptr(self._cell_start), ptr(self._cell_size), ptr(norms),
-                                     _lib.METRIC[self.distance], ptr(cells), ptr(n_probe_list), n_probe,
-                                     int(bool(self.use_smart_probing)), float(self.smart_probing_temperature), k,
-                                     ptr(self._address2id), ptr(values), ptr(ids), ptr(address), ptr(ws), ws_bytes,
-                                     _lib.current_stream(dev)))
+        entry, store = self._search_entry()
+        check(entry(ptr(x), self.d_vector, nq, ptr(vq), self.n_cells, *store, self.capacity,
+                    ptr(self._is_empty), ptr(self._cell_start), ptr(self._cell_size), ptr(norms),
+                    _lib.METRIC[self.distance], ptr(cells), ptr(n_probe_list), n_probe,
+                    int(bool(self.use_smart_probing)), float(self.smart_probing_temperature), k,
+                    ptr(self._address2id), ptr(values), ptr(ids), ptr(address), ptr(ws), ws_bytes,
+                    _lib.current_stream(dev)))
         return out
+
+    def _search_entry(self):
+        """(the library's search entry point, its store arguments between n_cells and capacity)."""
+        return lib.tpq_ivfflat_search, (ptr(self._storage),)
 
     def search(self, x, k=1, return_address=False):
         """x [d_vector, n_query] fp32 on the index device -> (values [n_query, k] fp32 descending, ids [n_query, k]
