@@ -217,6 +217,44 @@ int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* vq_codebook,
                      float temperature, int k, const int64_t* address2id, float* values, int64_t* ids,
                      int64_t* address, void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ range search (FlatIndex, IVFFlatIndex, IVFSQIndex)
+ * Every scored item whose score is above the threshold: the same items and scores as the searches above (tpq_flat_search's
+ * columns [0, n); the IVF searches' live slots of the visited cells), matched when score > threshold, strictly, in fp32
+ * (a NaN score never matches; +-inf thresholds are allowed, a NaN threshold is TPQ_ERR_BAD_ARG).
+ * -> match_keys [cap] u64 and match_query [cap] i32, unordered: one entry per match, match_query its query and match_keys
+ *   (order-preserving image of the fp32 score << 32) | (0xFFFFFFFF - address), the key every top-k here sorts by (key
+ *   descending = score descending, then address ascending; the image of f is bits(f) | 2^31 for f >= +0 and ~bits(f)
+ *   below).  *total (one u64 on the device) receives the exact count of matches; at most cap are written, the first
+ *   cap in no defined order, and nothing past cap.  A caller whose *total exceeds cap runs the call again with
+ *   cap >= *total; the result does not depend on the plan, the chunking or the batch.  cap == 0 counts only, and the
+ *   match arrays may then be NULL.  Arguments are checked before any launch; nq == 0 returns at once without writing
+ *   *total; n == 0 (capacity == 0) sets *total = 0.
+ * tpq_flat_range_search: over tpq_flat_search's store, metrics EUCLIDEAN, COSINE, INNER.  ws: at least
+ *   tpq_flat_range_workspace_bytes(d, nq, n) bytes.
+ * tpq_ivfflat_range_search / tpq_ivfsq_range_search: over tpq_ivfflat_search's / tpq_ivfsq_search's store, probe and
+ *   visiting rule, metrics EUCLIDEAN and COSINE.  A cell is visited at most once per query when cells == NULL (the
+ *   coarse probe returns distinct cells).  ws: at least tpq_ivfflat_range_workspace_bytes(d, nq, n_cells, n_probe)
+ *   bytes, which stops growing with nq past one chunk of queries (the most whose gathered pair queries, n_probe * d
+ *   floats each, fit 256 MB, at most 16 384). */
+size_t tpq_flat_range_workspace_bytes(int d, int nq, int64_t n);
+int tpq_flat_range_search(const float* x_dn, int d, int nq, const float* base, int64_t ld, int64_t n,
+                          const float* norms, int metric, float threshold, uint64_t* match_keys, int32_t* match_query,
+                          int64_t cap, uint64_t* total, void* ws, size_t ws_bytes, void* stream);
+size_t tpq_ivfflat_range_workspace_bytes(int d, int nq, int n_cells, int n_probe);
+int tpq_ivfflat_range_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                             const float* storage, int64_t capacity, const uint8_t* is_empty,
+                             const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
+                             const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart,
+                             float temperature, float threshold, uint64_t* match_keys, int32_t* match_query,
+                             int64_t cap, uint64_t* total, void* ws, size_t ws_bytes, void* stream);
+int tpq_ivfsq_range_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                           const uint8_t* storage, int bits, const float* lower, const float* range, int64_t capacity,
+                           const uint8_t* is_empty, const int64_t* cell_start, const int64_t* cell_size,
+                           const float* norms, int metric, const int64_t* cells, const int64_t* n_probe_list,
+                           int n_probe, int smart, float temperature, float threshold, uint64_t* match_keys,
+                           int32_t* match_query, int64_t cap, uint64_t* total, void* ws, size_t ws_bytes,
+                           void* stream);
+
 /* ------------------------------------------------------------------ row-wise top-k (fn.Topk, fn/Topk.py:43-67)
  * x [m, n] row-major, contiguous, fp32 or fp16 (dtype TPQ_DTYPE_*) -> the k best entries of every row: values [m, k]
  * f32 (an fp16 value widened exactly), indices [m, k] i64 (the column).  Order: value descending, then column

@@ -92,6 +92,13 @@ SIGNATURES = {
     "tpq_sq_decode": (_I, [_P, _I, _I64, _I, _P, _P, _P, _P]),
     "tpq_ivfsq_search": (_I, [_P, _I, _I, _P, _I, _P, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P, _P, _I, _I, _F, _I,
                               _P, _P, _P, _P, _P, _SZ, _P]),
+    "tpq_flat_range_workspace_bytes": (_SZ, [_I, _I, _I64]),
+    "tpq_flat_range_search": (_I, [_P, _I, _I, _P, _I64, _I64, _P, _I, _F, _P, _P, _I64, _P, _P, _SZ, _P]),
+    "tpq_ivfflat_range_workspace_bytes": (_SZ, [_I, _I, _I, _I]),
+    "tpq_ivfflat_range_search": (_I, [_P, _I, _I, _P, _I, _P, _I64, _P, _P, _P, _P, _I, _P, _P, _I, _I, _F, _F, _P,
+                                      _P, _I64, _P, _P, _SZ, _P]),
+    "tpq_ivfsq_range_search": (_I, [_P, _I, _I, _P, _I, _P, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P, _P, _I, _I, _F,
+                                    _F, _P, _P, _I64, _P, _P, _SZ, _P]),
 }
 
 DTYPE_F32, DTYPE_F16 = 0, 1     # TPQ_DTYPE_* (include/tpq_b200.h)

@@ -5,6 +5,7 @@
 // and one slice of the base columns; it writes its queries' sorted top-k keys to ws[slice, q, :], and
 // tpq_merge_topk merges the slices and decodes values, addresses and ids.
 #include "gemm_tile.cuh"
+#include "range.cuh"
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k, const int64_t* address2id,
                               int64_t capacity, float* values, int64_t* ids, int64_t* address, void* stream);
@@ -137,6 +138,102 @@ static bool flat_metric(int metric) {
   return metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE || metric == TPQ_METRIC_INNER;
 }
 
+// ----------------------------------------------------------------------------- range search
+// Shared memory of one range CTA: GEMM stages | match buffer (range.cuh).  QT = 64: 24 + 81 = 105 KB, two CTAs per SM.
+static size_t flat_range_smem_bytes(int qt) { return 2 * (size_t)GK * (qt + GB) * 4 + sizeof(RangeBuf); }
+
+// The plan of tpq_flat_range_search: QT and S as plan_flat's (no lists, so QT never halves); the workspace is |x|^2 and
+// the normalised queries.
+struct FlatRangePlan {
+  int qt, qtiles, S;
+  int64_t slice_cols;
+  size_t smem, xn, xq, total;
+};
+
+static FlatRangePlan plan_flat_range(int d, int nq, int64_t n) {
+  FlatRangePlan P{};
+  P.qt = 16;
+  while (P.qt < 64 && P.qt < nq) P.qt *= 2;
+  P.smem = flat_range_smem_bytes(P.qt);
+  P.qtiles = (nq + P.qt - 1) / P.qt;
+  const int64_t tiles = (n + GB - 1) / GB;
+  int64_t S = (2 * (int64_t)device_sm_count() + P.qtiles - 1) / P.qtiles;
+  S = S < 1 ? 1 : (tiles > 0 && S > tiles ? tiles : S);
+  const int64_t per = tiles > 0 ? (tiles + S - 1) / S : 1;
+  P.S = tiles > 0 ? (int)((tiles + per - 1) / per) : 1;
+  P.slice_cols = per * GB;
+  P.xn = 0;
+  P.xq = align_up((size_t)nq * 4, 256);
+  P.total = P.xq + align_up((size_t)d * nq * 4, 256);
+  return P;
+}
+
+// grid (query tiles, slices), 256 threads.  flat_search_kernel's GEMM and epilogue, then every score > thr (strict, in
+// fp32; NaN never passes) of a live column goes to the match buffer as (query, key); at most `cap` of them are written
+// to keys_out / q_out, and *total counts them all.
+template <int QT, int METRIC>
+__global__ void __launch_bounds__(256, 2)
+flat_range_kernel(const float* __restrict__ x, int d, int nq, const float* __restrict__ base, int64_t ld, int64_t n,
+                  const float* __restrict__ norms, const float* __restrict__ xn, float thr, int64_t slice_cols,
+                  uint64_t* __restrict__ keys_out, int32_t* __restrict__ q_out, int64_t cap,
+                  unsigned long long* __restrict__ total) {
+  using G = GemmTile<QT>;
+  extern __shared__ __align__(16) uint8_t smem[];
+  auto& stages = *reinterpret_cast<typename G::Stages*>(smem);
+  RangeBuf& mb = *reinterpret_cast<RangeBuf*>(smem + sizeof(typename G::Stages));
+  const int tid = threadIdx.x, lane = tid & 31, tx = tid & 15, ty = tid >> 4;
+  const int q0 = blockIdx.x * QT;
+  const int64_t c_begin = (int64_t)blockIdx.y * slice_cols;
+  const int64_t c_end = c_begin + slice_cols < n ? c_begin + slice_cols : n;
+  auto query = [&](int r) { return q0 + r; };
+  if (tid == 0) mb.cnt = 0;                            // ordered before the first append by G::run's first barrier
+  for (int64_t c0 = c_begin; c0 < c_end; c0 += GB) {
+    float acc[G::MI][8];
+    G::run(x, nq, q0, base + c0, ld, (int)(c_end - c0 < GB ? c_end - c0 : GB), d, stages, acc);
+    float nc[8];
+    #pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int64_t c = c0 + G::col(j, tx);
+      nc[j] = (METRIC != TPQ_METRIC_INNER && c < c_end) ? norms[c] : 1.f;
+    }
+    uint32_t pass = 0;
+    #pragma unroll
+    for (int i = 0; i < G::MI; ++i) {
+      const int r = G::row(i, ty);
+      const float a2 = (METRIC == TPQ_METRIC_EUCLIDEAN && q0 + r < nq) ? xn[q0 + r] : 0.f;
+      #pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float o;
+        if (METRIC == TPQ_METRIC_EUCLIDEAN) o = __fsub_rn(__fsub_rn(__fmul_rn(acc[i][j], 2.f), a2), nc[j]);
+        else if (METRIC == TPQ_METRIC_COSINE) o = __fdiv_rn(acc[i][j], nc[j]);
+        else o = acc[i][j];
+        acc[i][j] = o;
+        if (q0 + r < nq && c0 + G::col(j, tx) < c_end && o > thr) pass |= 1u << (i * 8 + j);
+      }
+    }
+    range_append(mb, pass, acc, [&](int i) { return G::row(i, ty); },
+                 [&](int j) { return (uint32_t)(c0 + G::col(j, tx)); }, lane);
+    __syncthreads();                                   // the appends, and this tile's last reads of the stages
+    if (mb.cnt > kRangeBuf - QT * GB) range_flush(mb, total, cap, keys_out, q_out, query);
+  }
+  __syncthreads();
+  range_flush(mb, total, cap, keys_out, q_out, query);
+}
+
+template <int QT>
+static int launch_flat_range(int metric, const FlatRangePlan& P, const float* x, int d, int nq, const float* base,
+                             int64_t ld, int64_t n, const float* norms, const float* xn, float thr, uint64_t* keys,
+                             int32_t* query, int64_t cap, unsigned long long* total, cudaStream_t st) {
+  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? flat_range_kernel<QT, TPQ_METRIC_EUCLIDEAN>
+            : metric == TPQ_METRIC_COSINE    ? flat_range_kernel<QT, TPQ_METRIC_COSINE>
+                                             : flat_range_kernel<QT, TPQ_METRIC_INNER>;
+  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
+  kern<<<dim3(P.qtiles, P.S), 256, P.smem, st>>>(x, d, nq, base, ld, n, norms, xn, thr, P.slice_cols, keys, query, cap,
+                                                 total);
+  TPQ_LAUNCH_CHECK("flat_range_kernel");
+  return TPQ_OK;
+}
+
 }  // namespace tpq
 
 using namespace tpq;
@@ -197,4 +294,55 @@ extern "C" int tpq_flat_search(const float* x_dn, int d, int nq, const float* ba
   // n == 0: every key is empty and the id table (capacity 0) is never read, so any non-null pointer will do
   return tpq_merge_topk(keys, nq, P.S, k, n ? address2id : reinterpret_cast<const int64_t*>(keys), n, values, ids,
                         address, stream);
+}
+
+extern "C" size_t tpq_flat_range_workspace_bytes(int d, int nq, int64_t n) {
+  if (d <= 0 || nq <= 0 || n < 0) return 0;
+  return plan_flat_range(d, nq, n).total;
+}
+
+extern "C" int tpq_flat_range_search(const float* x_dn, int d, int nq, const float* base, int64_t ld, int64_t n,
+                                     const float* norms, int metric, float threshold, uint64_t* match_keys,
+                                     int32_t* match_query, int64_t cap, uint64_t* total, void* ws, size_t ws_bytes,
+                                     void* stream) {
+  if (!flat_metric(metric)) {
+    set_error("tpq_flat_range_search: unsupported metric %d", metric);
+    return TPQ_ERR_UNSUPPORTED;
+  }
+  TPQ_REQUIRE(threshold == threshold, "tpq_flat_range_search: the threshold is NaN");
+  TPQ_REQUIRE(d > 0 && nq >= 0 && n >= 0 && ld >= n && cap >= 0,
+              "tpq_flat_range_search: bad sizes d=%d nq=%d n=%lld ld=%lld cap=%lld", d, nq, (long long)n, (long long)ld,
+              (long long)cap);
+  TPQ_REQUIRE(n < (int64_t(1) << 32), "tpq_flat_range_search: n=%lld exceeds the 32-bit address of a key", (long long)n);
+  TPQ_REQUIRE(total && (cap == 0 || (match_keys && match_query)), "tpq_flat_range_search: null total or match buffer");
+  if (nq == 0) return TPQ_OK;
+  TPQ_REQUIRE(x_dn, "tpq_flat_range_search: null query pointer");
+  TPQ_REQUIRE(n == 0 || (base && (norms || metric == TPQ_METRIC_INNER)), "tpq_flat_range_search: null base or norms");
+  const FlatRangePlan P = plan_flat_range(d, nq, n);
+  if (!ws || ws_bytes < P.total) {
+    set_error("tpq_flat_range_search: workspace too small (%zu < %zu)", ws_bytes, P.total);
+    return TPQ_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  TPQ_CUDA(cudaMemsetAsync(total, 0, sizeof(uint64_t), st));
+  if (n == 0) return TPQ_OK;
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  float* xn = reinterpret_cast<float*>(w + P.xn);
+  const float* xq = x_dn;
+  if (metric == TPQ_METRIC_EUCLIDEAN) {
+    if (int rc = col_sqnorms(x_dn, d, nq, nq, xn, st)) return rc;
+  } else if (metric == TPQ_METRIC_COSINE) {
+    float* xs = reinterpret_cast<float*>(w + P.xq);
+    if (int rc = normalize_columns(x_dn, d, nq, kFlatEps, xs, st)) return rc;
+    xq = xs;
+  }
+  unsigned long long* t = reinterpret_cast<unsigned long long*>(total);
+  switch (P.qt) {
+    case 16: return launch_flat_range<16>(metric, P, xq, d, nq, base, ld, n, norms, xn, threshold, match_keys,
+                                          match_query, cap, t, st);
+    case 32: return launch_flat_range<32>(metric, P, xq, d, nq, base, ld, n, norms, xn, threshold, match_keys,
+                                          match_query, cap, t, st);
+    default: return launch_flat_range<64>(metric, P, xq, d, nq, base, ld, n, norms, xn, threshold, match_keys,
+                                          match_query, cap, t, st);
+  }
 }

@@ -24,6 +24,7 @@
 // stages them, so its scores are this search's over the decoded store, bit for bit.
 #include "gemm_tile.cuh"
 #include "scan_layout.cuh"
+#include "range.cuh"
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k, const int64_t* address2id,
                               int64_t capacity, float* values, int64_t* ids, int64_t* address, void* stream);
@@ -274,6 +275,128 @@ ivfflat_scan_kernel(const float* __restrict__ xg, int d, int pad_cap, const int*
   }
 }
 
+// ----------------------------------------------------------------------------- range search
+// tpq_ivfflat_range_search / tpq_ivfsq_range_search run steps 1-4 of every chunk as the search does, then
+// ivfflat_range_kernel, which keeps no lists: the scores above the threshold go to the match buffer of range.cuh.
+constexpr size_t kIvfRangeXgBytes = size_t(256) << 20;   // the chunk's gathered pair queries stay within 256 MB
+
+// Shared memory of one range CTA: GEMM stages | match buffer.  QT = 64: 24 + 81 = 105 KB, two CTAs per SM.
+static size_t ivfflat_range_smem_bytes(int qt) { return 2 * (size_t)GK * (qt + GB) * 4 + sizeof(RangeBuf); }
+
+// The range search's plan, read by its workspace size and the launches; the search's layout without keys:
+//   chunk: queries per chunk, the most whose n_probe pair columns of d floats fit kIvfRangeXgBytes, at most
+//          kIvfFlatMaxChunk -- the workspace stops growing with nq past one chunk;
+//   QT, S: as plan_ivfflat's for this chunk (no lists, so QT never halves).
+static IvfFlatPlan plan_ivfflat_range(int d, int nq, int n_cells, int n_probe) {
+  IvfFlatPlan P{};
+  size_t c = kIvfRangeXgBytes / ((size_t)n_probe * d * 4);
+  c = c < (size_t)kIvfFlatMaxChunk ? c : (size_t)kIvfFlatMaxChunk;
+  P.chunk = (int)(c < 1 ? 1 : (c > (size_t)nq ? (size_t)nq : c));
+  const int64_t per_cell = ((int64_t)P.chunk * n_probe + n_cells - 1) / n_cells;
+  P.qt = 16;
+  while (P.qt < 64 && P.qt < per_cell) P.qt *= 2;
+  P.smem = ivfflat_range_smem_bytes(P.qt);
+  const int64_t tiles = ((int64_t)P.chunk * n_probe + P.qt - 1) / P.qt;
+  const int64_t want = 2 * (int64_t)device_sm_count();
+  const int smax = n_probe >= kIvfFlatMaxSlices ? 1 : kIvfFlatMaxSlices / n_probe;
+  const int64_t S = tiles >= want ? 1 : (want + tiles - 1) / tiles;
+  P.S = (int)(S > smax ? smax : S);
+  P.pairs = (int64_t)P.chunk * n_probe;
+  P.pad_cap = P.pairs + (P.pairs < n_cells ? P.pairs : n_cells) * (P.qt - 1);
+  P.items = P.S * (P.pad_cap / P.qt);
+  const size_t n = (size_t)P.chunk;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t at = o; o += align_up(bytes, 256); return at; };
+  P.xc = take((size_t)d * n * 4);
+  P.xs = take((size_t)d * n * 4);
+  P.xp = take((size_t)d * n * 4);
+  P.xn = take(n * 4);
+  P.coarse_bytes = tpq_coarse_workspace_bytes(d, (int)n, n_cells);
+  P.coarse = take(P.coarse_bytes);
+  P.sims = take(n * n_probe * 4);
+  P.cells = take(n * n_probe * 8);
+  P.npl = take(n * 8);
+  P.cnt = take(((size_t)n_cells + 2) * 4);
+  P.off = take((size_t)n_cells * 4);
+  P.slot = take((size_t)P.pairs * 4);
+  P.pq = take((size_t)P.pad_cap * 4);
+  P.pj = take((size_t)P.pad_cap * 4);
+  P.itm = take((size_t)P.items * 16);
+  P.xg = take((size_t)d * P.pad_cap * 4);
+  P.total = o;
+  return P;
+}
+
+// One CTA per work item, as ivfflat_scan_kernel: the same GEMM, epilogue and is_empty mask, then every score > thr
+// (strict, in fp32; NaN never passes) goes to the match buffer as (pair row, key); a flush maps the row to its query,
+// q_base + pair_q[row], writes at most `cap` matches to keys_out / q_out and counts them all in *total.
+template <int QT, int METRIC, class BL, class... Extra>
+__global__ void __launch_bounds__(256, 2)
+ivfflat_range_kernel(const float* __restrict__ xg, int d, int pad_cap, const int* __restrict__ pair_q,
+                     const int4* __restrict__ items, const int* __restrict__ cnt, int n_cells,
+                     const int* __restrict__ off, const typename BL::T* __restrict__ base, int64_t ld,
+                     const uint8_t* __restrict__ is_empty, const int64_t* __restrict__ cell_start,
+                     const int64_t* __restrict__ cell_size, const float* __restrict__ norms,
+                     const float* __restrict__ xn, int S, float thr, int q_base, uint64_t* __restrict__ keys_out,
+                     int32_t* __restrict__ q_out, int64_t cap, unsigned long long* __restrict__ total,
+                     Extra... extra) {
+  using G = GemmTile<QT, BL>;
+  if ((int)blockIdx.x >= cnt[n_cells]) return;
+  const int4 it = items[blockIdx.x];
+  const int cell = it.x, sl = it.z;
+  const int64_t size = cell_size[cell], start = cell_start[cell];
+  const int64_t T = (size + GB - 1) / GB;
+  const int64_t c_begin = start + T * sl / S * GB;
+  const int64_t c_end = start + (T * (sl + 1) / S * GB < size ? T * (sl + 1) / S * GB : size);
+  if (c_begin >= c_end) return;
+  const int p0 = off[cell] + it.y * QT;
+  const int rows = cnt[cell] - it.y * QT < QT ? cnt[cell] - it.y * QT : QT;
+  extern __shared__ __align__(16) uint8_t smem[];
+  auto& stages = *reinterpret_cast<typename G::Stages*>(smem);
+  RangeBuf& mb = *reinterpret_cast<RangeBuf*>(smem + sizeof(typename G::Stages));
+  const int tid = threadIdx.x, lane = tid & 31, tx = tid & 15, ty = tid >> 4;
+  float a2[G::MI];
+  #pragma unroll
+  for (int i = 0; i < G::MI; ++i) {
+    const int r = G::row(i, ty);
+    a2[i] = (METRIC == TPQ_METRIC_EUCLIDEAN && r < rows) ? xn[pair_q[p0 + r]] : 0.f;
+  }
+  auto query = [&](int r) { return q_base + pair_q[p0 + r]; };
+  if (tid == 0) mb.cnt = 0;                            // ordered before the first append by G::run's first barrier
+  for (int64_t c0 = c_begin; c0 < c_end; c0 += GB) {
+    const int cols = (int)(c_end - c0 < GB ? c_end - c0 : GB);
+    float acc[G::MI][8];
+    G::run(xg, pad_cap, p0, BL{base + c0, ld, extra...}, cols, d, stages, acc);
+    float nc[8];
+    bool live[8];
+    #pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = G::col(j, tx);
+      live[j] = c < cols && is_empty[c0 + c] == 0;
+      nc[j] = c < cols ? norms[c0 + c] : 1.f;
+    }
+    uint32_t pass = 0;
+    #pragma unroll
+    for (int i = 0; i < G::MI; ++i) {
+      const bool row_ok = G::row(i, ty) < rows;
+      #pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float o;
+        if (METRIC == TPQ_METRIC_EUCLIDEAN) o = __fsub_rn(__fsub_rn(__fmul_rn(acc[i][j], 2.f), a2[i]), nc[j]);
+        else o = __fdiv_rn(acc[i][j], nc[j]);
+        acc[i][j] = o;
+        if (row_ok && live[j] && o > thr) pass |= 1u << (i * 8 + j);
+      }
+    }
+    range_append(mb, pass, acc, [&](int i) { return G::row(i, ty); },
+                 [&](int j) { return (uint32_t)(c0 + G::col(j, tx)); }, lane);
+    __syncthreads();                                   // the appends, and this tile's last reads of the stages
+    if (mb.cnt > kRangeBuf - QT * GB) range_flush(mb, total, cap, keys_out, q_out, query);
+  }
+  __syncthreads();
+  range_flush(mb, total, cap, keys_out, q_out, query);
+}
+
 }  // namespace tpq
 
 using namespace tpq;
@@ -281,6 +404,91 @@ using namespace tpq;
 extern "C" size_t tpq_ivfflat_workspace_bytes(int d, int nq, int n_cells, int n_probe, int k) {
   if (d <= 0 || nq <= 0 || n_cells <= 0 || n_probe <= 0 || k <= 0 || k > 1024) return 0;
   return plan_ivfflat(d, nq, n_cells, n_probe, k).total;
+}
+
+// The chunk's part of the workspace, at the plan's offsets.
+struct IvfChunk {
+  float *xc, *xs, *xp, *xn, *xg;
+  int *cnt, *off, *slot, *pair_q, *pair_j;
+  int4* items;
+};
+
+static IvfChunk ivf_chunk_ws(const IvfFlatPlan& P, uint8_t* w) {
+  IvfChunk W;
+  W.xc = reinterpret_cast<float*>(w + P.xc); W.xs = reinterpret_cast<float*>(w + P.xs);
+  W.xp = reinterpret_cast<float*>(w + P.xp); W.xn = reinterpret_cast<float*>(w + P.xn);
+  W.xg = reinterpret_cast<float*>(w + P.xg);
+  W.cnt = reinterpret_cast<int*>(w + P.cnt); W.off = reinterpret_cast<int*>(w + P.off);
+  W.slot = reinterpret_cast<int*>(w + P.slot); W.pair_q = reinterpret_cast<int*>(w + P.pq);
+  W.pair_j = reinterpret_cast<int*>(w + P.pj);
+  W.items = reinterpret_cast<int4*>(w + P.itm);
+  return W;
+}
+
+// Steps 1-4 of the chunk [q0, q0 + n) of the batch, shared by the search and the range search: the chunk's queries, its
+// probe lists (the caller's, or the coarse probe's), |x|^2 (euclidean) or the normalised queries (cosine), the visited
+// pairs grouped by cell, the work items and the pairs' queries gathered into W.xg.
+static int ivf_chunk_pairs(const IvfFlatPlan& P, uint8_t* w, const IvfChunk& W, const float* x_dn, int d, int nq, int q0,
+                           int n, const float* vq_codebook, int n_cells, const int64_t* cells,
+                           const int64_t* n_probe_list, int n_probe, int smart, float temperature, int metric,
+                           const int64_t* cell_start, const int64_t* cell_size, cudaStream_t st) {
+  void* stream = st;
+  float *xc = W.xc, *xs = W.xs, *xp = W.xp, *xn = W.xn;
+  TPQ_CUDA(cudaMemcpy2DAsync(xc, (size_t)n * 4, x_dn + q0, (size_t)nq * 4, (size_t)n * 4, d, cudaMemcpyDeviceToDevice, st));
+  const int64_t *cq = cells ? cells + (size_t)q0 * n_probe : nullptr, *npl = cells ? n_probe_list + q0 : nullptr;
+  if (!cells) {                                        // tpq_ivfpq_search's coarse stage, on the chunk
+    const float* xprobe = xc;
+    if (metric == TPQ_METRIC_COSINE) {
+      if (int rc = tpq_normalize_columns(xc, d, n, xp, stream)) return rc;
+      xprobe = xp;
+    }
+    int64_t *cw = reinterpret_cast<int64_t*>(w + P.cells), *nw = reinterpret_cast<int64_t*>(w + P.npl);
+    if (int rc = tpq_coarse_probe(xprobe, vq_codebook, d, n, n_cells, n_probe, smart, temperature,
+                                  reinterpret_cast<float*>(w + P.sims), cw, nw, w + P.coarse, P.coarse_bytes, stream))
+      return rc;
+    cq = cw; npl = nw;
+  }
+  const float* xq = xc;
+  if (metric == TPQ_METRIC_EUCLIDEAN) {
+    if (int rc = col_sqnorms(xc, d, n, n, xn, st)) return rc;
+  } else {
+    if (int rc = normalize_columns(xc, d, n, kIvfFlatEps, xs, st)) return rc;
+    xq = xs;
+  }
+  const int64_t nt = (int64_t)n * n_probe;
+  const unsigned pgrid = (unsigned)((nt + 255) / 256);
+  TPQ_CUDA(cudaMemsetAsync(W.cnt, 0, ((size_t)n_cells + 2) * 4, st));
+  TPQ_CUDA(cudaMemsetAsync(W.pair_q, 0xFF, (size_t)P.pad_cap * 4, st));
+  ivfflat_pairs_count_kernel<<<pgrid, 256, 0, st>>>(cq, npl, n, n_probe, n_cells, cell_start, cell_size, W.cnt, W.slot);
+  TPQ_LAUNCH_CHECK("ivfflat_pairs_count_kernel");
+  ivfflat_plan_kernel<<<1, 1024, 0, st>>>(W.cnt, cell_size, n_cells, P.qt, P.S, W.off, W.items);
+  TPQ_LAUNCH_CHECK("ivfflat_plan_kernel");
+  ivfflat_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(cq, n, n_probe, W.slot, W.off, W.pair_q, W.pair_j);
+  TPQ_LAUNCH_CHECK("ivfflat_pairs_scatter_kernel");
+  const dim3 ggrid((unsigned)((P.pad_cap + 255) / 256), (unsigned)(d < 64 ? d : 64));
+  ivfflat_gather_kernel<<<ggrid, 256, 0, st>>>(xq, d, n, W.pair_q, W.cnt + n_cells + 1, P.pad_cap, W.xg);
+  TPQ_LAUNCH_CHECK("ivfflat_gather_kernel");
+  return TPQ_OK;
+}
+
+// The checks of the search and the range search on the metric, the sizes and the probe lists.
+static int ivf_check(const char* name, int d, int nq, int n_cells, int n_probe, int64_t capacity, int metric,
+                     const int64_t* cells, const int64_t* n_probe_list) {
+  if (metric != TPQ_METRIC_EUCLIDEAN && metric != TPQ_METRIC_COSINE) {
+    set_error("%s: unsupported metric %d (euclidean and cosine only)", name, metric);
+    return TPQ_ERR_UNSUPPORTED;
+  }
+  TPQ_REQUIRE(d > 0 && nq >= 0 && n_cells > 0 && n_probe >= 1 && capacity >= 0,
+              "%s: bad sizes d=%d nq=%d n_cells=%d n_probe=%d capacity=%lld", name, d, nq, n_cells, n_probe,
+              (long long)capacity);
+  TPQ_REQUIRE(capacity < (int64_t(1) << 32), "%s: capacity=%lld exceeds the 32-bit address of a key", name,
+              (long long)capacity);
+  TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "%s: cells and n_probe_list go together", name);
+  if (!cells) {
+    TPQ_REQUIRE(n_probe <= n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, n_cells);
+    if (n_probe > 1024) { set_error("n_probe=%d > 1024 is not supported", n_probe); return TPQ_ERR_UNSUPPORTED; }
+  }
+  return TPQ_OK;
 }
 
 template <int QT, class BL, class... Extra>
@@ -310,20 +518,7 @@ static int ivf_search(const char* name, const float* x_dn, int d, int nq, const 
                       size_t ws_bytes, void* stream, Extra... extra) {
   TPQ_REQUIRE(k > 0, "k must be in (0, 1024], got %d", k);
   if (k > 1024) { set_error("k=%d > 1024 is not supported", k); return TPQ_ERR_UNSUPPORTED; }
-  if (metric != TPQ_METRIC_EUCLIDEAN && metric != TPQ_METRIC_COSINE) {
-    set_error("%s: unsupported metric %d (euclidean and cosine only)", name, metric);
-    return TPQ_ERR_UNSUPPORTED;
-  }
-  TPQ_REQUIRE(d > 0 && nq >= 0 && n_cells > 0 && n_probe >= 1 && capacity >= 0,
-              "%s: bad sizes d=%d nq=%d n_cells=%d n_probe=%d capacity=%lld", name, d, nq, n_cells, n_probe,
-              (long long)capacity);
-  TPQ_REQUIRE(capacity < (int64_t(1) << 32), "%s: capacity=%lld exceeds the 32-bit address of a key", name,
-              (long long)capacity);
-  TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "%s: cells and n_probe_list go together", name);
-  if (!cells) {
-    TPQ_REQUIRE(n_probe <= n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, n_cells);
-    if (n_probe > 1024) { set_error("n_probe=%d > 1024 is not supported", n_probe); return TPQ_ERR_UNSUPPORTED; }
-  }
+  if (int rc = ivf_check(name, d, nq, n_cells, n_probe, capacity, metric, cells, n_probe_list)) return rc;
   TPQ_REQUIRE(values && ids, "%s: null output", name);
   if (nq == 0) return TPQ_OK;
   TPQ_REQUIRE(x_dn && cell_start && cell_size && (cells || vq_codebook), "%s: null query or cell table", name);
@@ -336,52 +531,18 @@ static int ivf_search(const char* name, const float* x_dn, int d, int nq, const 
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
   uint64_t* keys = reinterpret_cast<uint64_t*>(w + P.keys);
-  float *xc = reinterpret_cast<float*>(w + P.xc), *xs = reinterpret_cast<float*>(w + P.xs);
-  float *xp = reinterpret_cast<float*>(w + P.xp), *xn = reinterpret_cast<float*>(w + P.xn);
-  int *cnt = reinterpret_cast<int*>(w + P.cnt), *off = reinterpret_cast<int*>(w + P.off);
-  int *slot = reinterpret_cast<int*>(w + P.slot), *pair_q = reinterpret_cast<int*>(w + P.pq);
-  int* pair_j = reinterpret_cast<int*>(w + P.pj);
-  int4* items = reinterpret_cast<int4*>(w + P.itm);
-  float* xg = reinterpret_cast<float*>(w + P.xg);
+  const IvfChunk W = ivf_chunk_ws(P, w);
+  float *xn = W.xn, *xg = W.xg;
+  int *cnt = W.cnt, *off = W.off, *pair_q = W.pair_q, *pair_j = W.pair_j;
+  int4* items = W.items;
   // capacity == 0: every key is empty and the id table is never read, so any non-null pointer will do
   const int64_t* a2i = capacity ? address2id : reinterpret_cast<const int64_t*>(keys);
   for (int q0 = 0; q0 < nq; q0 += P.chunk) {
     const int n = nq - q0 < P.chunk ? nq - q0 : P.chunk;
-    TPQ_CUDA(cudaMemcpy2DAsync(xc, (size_t)n * 4, x_dn + q0, (size_t)nq * 4, (size_t)n * 4, d, cudaMemcpyDeviceToDevice, st));
-    const int64_t *cq = cells ? cells + (size_t)q0 * n_probe : nullptr, *npl = cells ? n_probe_list + q0 : nullptr;
-    if (!cells) {                                      // tpq_ivfpq_search's coarse stage, on the chunk
-      const float* xprobe = xc;
-      if (metric == TPQ_METRIC_COSINE) {
-        if (int rc = tpq_normalize_columns(xc, d, n, xp, stream)) return rc;
-        xprobe = xp;
-      }
-      int64_t *cw = reinterpret_cast<int64_t*>(w + P.cells), *nw = reinterpret_cast<int64_t*>(w + P.npl);
-      if (int rc = tpq_coarse_probe(xprobe, vq_codebook, d, n, n_cells, n_probe, smart, temperature,
-                                    reinterpret_cast<float*>(w + P.sims), cw, nw, w + P.coarse, P.coarse_bytes, stream))
-        return rc;
-      cq = cw; npl = nw;
-    }
-    const float* xq = xc;
-    if (metric == TPQ_METRIC_EUCLIDEAN) {
-      if (int rc = col_sqnorms(xc, d, n, n, xn, st)) return rc;
-    } else {
-      if (int rc = normalize_columns(xc, d, n, kIvfFlatEps, xs, st)) return rc;
-      xq = xs;
-    }
-    const int64_t nt = (int64_t)n * n_probe;
-    const unsigned pgrid = (unsigned)((nt + 255) / 256);
-    TPQ_CUDA(cudaMemsetAsync(cnt, 0, ((size_t)n_cells + 2) * 4, st));
-    TPQ_CUDA(cudaMemsetAsync(pair_q, 0xFF, (size_t)P.pad_cap * 4, st));
     TPQ_CUDA(cudaMemsetAsync(keys, 0, (size_t)n_probe * P.S * n * k * 8, st));
-    ivfflat_pairs_count_kernel<<<pgrid, 256, 0, st>>>(cq, npl, n, n_probe, n_cells, cell_start, cell_size, cnt, slot);
-    TPQ_LAUNCH_CHECK("ivfflat_pairs_count_kernel");
-    ivfflat_plan_kernel<<<1, 1024, 0, st>>>(cnt, cell_size, n_cells, P.qt, P.S, off, items);
-    TPQ_LAUNCH_CHECK("ivfflat_plan_kernel");
-    ivfflat_pairs_scatter_kernel<<<pgrid, 256, 0, st>>>(cq, n, n_probe, slot, off, pair_q, pair_j);
-    TPQ_LAUNCH_CHECK("ivfflat_pairs_scatter_kernel");
-    const dim3 ggrid((unsigned)((P.pad_cap + 255) / 256), (unsigned)(d < 64 ? d : 64));
-    ivfflat_gather_kernel<<<ggrid, 256, 0, st>>>(xq, d, n, pair_q, cnt + n_cells + 1, P.pad_cap, xg);
-    TPQ_LAUNCH_CHECK("ivfflat_gather_kernel");
+    if (int rc = ivf_chunk_pairs(P, w, W, x_dn, d, nq, q0, n, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart,
+                                 temperature, metric, cell_start, cell_size, st))
+      return rc;
     int rc;
     switch (P.qt) {
       case 16: rc = launch_ivfflat_scan<16, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
@@ -437,4 +598,112 @@ extern "C" int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* v
   return ivf_search<BLoadSQ8>("tpq_ivfsq_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
                               cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart, temperature,
                               k, address2id, values, ids, address, ws, ws_bytes, stream, lower, range);
+}
+
+// ----------------------------------------------------------------------------- range search
+extern "C" size_t tpq_ivfflat_range_workspace_bytes(int d, int nq, int n_cells, int n_probe) {
+  if (d <= 0 || nq <= 0 || n_cells <= 0 || n_probe <= 0) return 0;
+  return plan_ivfflat_range(d, nq, n_cells, n_probe).total;
+}
+
+template <int QT, class BL, class... Extra>
+static int launch_ivfflat_range(int metric, const IvfFlatPlan& P, const IvfChunk& W, int d, int n_cells,
+                                const typename BL::T* storage, int64_t capacity, const uint8_t* is_empty,
+                                const int64_t* cell_start, const int64_t* cell_size, const float* norms, float thr,
+                                int q_base, uint64_t* keys, int32_t* query, int64_t cap, unsigned long long* total,
+                                cudaStream_t st, Extra... extra) {
+  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? ivfflat_range_kernel<QT, TPQ_METRIC_EUCLIDEAN, BL, Extra...>
+                                             : ivfflat_range_kernel<QT, TPQ_METRIC_COSINE, BL, Extra...>;
+  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
+  kern<<<(unsigned)P.items, 256, P.smem, st>>>(W.xg, d, (int)P.pad_cap, W.pair_q, W.items, W.cnt, n_cells, W.off,
+                                               storage, capacity, is_empty, cell_start, cell_size, norms, W.xn, P.S,
+                                               thr, q_base, keys, query, cap, total, extra...);
+  TPQ_LAUNCH_CHECK("ivfflat_range_kernel");
+  return TPQ_OK;
+}
+
+// The body of tpq_ivfflat_range_search and tpq_ivfsq_range_search, as ivf_search is of the searches.
+template <class BL, class... Extra>
+static int ivf_range(const char* name, const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                     const typename BL::T* storage, int64_t capacity, const uint8_t* is_empty,
+                     const int64_t* cell_start, const int64_t* cell_size, const float* norms, int metric,
+                     const int64_t* cells, const int64_t* n_probe_list, int n_probe, int smart, float temperature,
+                     float threshold, uint64_t* match_keys, int32_t* match_query, int64_t cap, uint64_t* total,
+                     void* ws, size_t ws_bytes, void* stream, Extra... extra) {
+  if (int rc = ivf_check(name, d, nq, n_cells, n_probe, capacity, metric, cells, n_probe_list)) return rc;
+  TPQ_REQUIRE(threshold == threshold, "%s: the threshold is NaN", name);
+  TPQ_REQUIRE(cap >= 0, "%s: cap=%lld is negative", name, (long long)cap);
+  TPQ_REQUIRE(total && (cap == 0 || (match_keys && match_query)), "%s: null total or match buffer", name);
+  if (nq == 0) return TPQ_OK;
+  TPQ_REQUIRE(x_dn && cell_start && cell_size && (cells || vq_codebook), "%s: null query or cell table", name);
+  TPQ_REQUIRE(capacity == 0 || (storage && is_empty && norms), "%s: null store", name);
+  const IvfFlatPlan P = plan_ivfflat_range(d, nq, n_cells, n_probe);
+  if (!ws || ws_bytes < P.total) {
+    set_error("%s: workspace too small (%zu < %zu)", name, ws_bytes, P.total);
+    return TPQ_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  TPQ_CUDA(cudaMemsetAsync(total, 0, sizeof(uint64_t), st));
+  if (capacity == 0) return TPQ_OK;                    // nothing to score
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  const IvfChunk W = ivf_chunk_ws(P, w);
+  unsigned long long* t = reinterpret_cast<unsigned long long*>(total);
+  for (int q0 = 0; q0 < nq; q0 += P.chunk) {
+    const int n = nq - q0 < P.chunk ? nq - q0 : P.chunk;
+    if (int rc = ivf_chunk_pairs(P, w, W, x_dn, d, nq, q0, n, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart,
+                                 temperature, metric, cell_start, cell_size, st))
+      return rc;
+    int rc;
+    switch (P.qt) {
+      case 16: rc = launch_ivfflat_range<16, BL>(metric, P, W, d, n_cells, storage, capacity, is_empty, cell_start,
+                                                 cell_size, norms, threshold, q0, match_keys, match_query, cap, t, st,
+                                                 extra...); break;
+      case 32: rc = launch_ivfflat_range<32, BL>(metric, P, W, d, n_cells, storage, capacity, is_empty, cell_start,
+                                                 cell_size, norms, threshold, q0, match_keys, match_query, cap, t, st,
+                                                 extra...); break;
+      default: rc = launch_ivfflat_range<64, BL>(metric, P, W, d, n_cells, storage, capacity, is_empty, cell_start,
+                                                 cell_size, norms, threshold, q0, match_keys, match_query, cap, t, st,
+                                                 extra...); break;
+    }
+    if (rc) return rc;
+  }
+  return TPQ_OK;
+}
+
+extern "C" int tpq_ivfflat_range_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                                        const float* storage, int64_t capacity, const uint8_t* is_empty,
+                                        const int64_t* cell_start, const int64_t* cell_size, const float* norms,
+                                        int metric, const int64_t* cells, const int64_t* n_probe_list, int n_probe,
+                                        int smart, float temperature, float threshold, uint64_t* match_keys,
+                                        int32_t* match_query, int64_t cap, uint64_t* total, void* ws, size_t ws_bytes,
+                                        void* stream) {
+  return ivf_range<BLoadF32>("tpq_ivfflat_range_search", x_dn, d, nq, vq_codebook, n_cells, storage, capacity,
+                             is_empty, cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
+                             temperature, threshold, match_keys, match_query, cap, total, ws, ws_bytes, stream);
+}
+
+extern "C" int tpq_ivfsq_range_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
+                                      const uint8_t* storage, int bits, const float* lower, const float* range,
+                                      int64_t capacity, const uint8_t* is_empty, const int64_t* cell_start,
+                                      const int64_t* cell_size, const float* norms, int metric, const int64_t* cells,
+                                      const int64_t* n_probe_list, int n_probe, int smart, float temperature,
+                                      float threshold, uint64_t* match_keys, int32_t* match_query, int64_t cap,
+                                      uint64_t* total, void* ws, size_t ws_bytes, void* stream) {
+  if (bits != 8 && bits != 16) {
+    set_error("tpq_ivfsq_range_search: bits=%d is not supported (8 and 16 only)", bits);
+    return TPQ_ERR_UNSUPPORTED;
+  }
+  TPQ_REQUIRE(d > 0 && d % (bits == 8 ? 4 : 2) == 0,
+              "tpq_ivfsq_range_search: d=%d must be a positive multiple of %d for %d bits", d, bits == 8 ? 4 : 2, bits);
+  const uint32_t* words = reinterpret_cast<const uint32_t*>(storage);
+  if (bits == 16)
+    return ivf_range<BLoadSQ16>("tpq_ivfsq_range_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity,
+                                is_empty, cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
+                                temperature, threshold, match_keys, match_query, cap, total, ws, ws_bytes, stream);
+  TPQ_REQUIRE(lower && range, "tpq_ivfsq_range_search: null lower or range (8 bits)");
+  TPQ_REQUIRE((reinterpret_cast<uintptr_t>(lower) | reinterpret_cast<uintptr_t>(range)) % 16 == 0,
+              "tpq_ivfsq_range_search: lower and range must be 16-byte aligned");
+  return ivf_range<BLoadSQ8>("tpq_ivfsq_range_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
+                             cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart, temperature,
+                             threshold, match_keys, match_query, cap, total, ws, ws_bytes, stream, lower, range);
 }

@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib
+from . import _lib, _range
 from ._lib import lib, check, ptr
 from .modules import IdContainer, _fingerprint
 
@@ -191,3 +191,32 @@ class FlatIndex(IdContainer):
                                   _lib.METRIC[self.distance], k, ptr(self._address2id), ptr(values), ptr(ids),
                                   ptr(address), ptr(ws), ws_bytes, _lib.current_stream(dev)))
         return out
+
+    def range_search(self, x, threshold, return_address=False, max_results=1 << 26):
+        """Every live item scoring above `threshold`: x [d_vector, n_query] fp32 on the index device, threshold a float
+        or a 0-d tensor (rounded once to fp32; NaN raises ValueError)
+        -> (lims [n_query + 1] int64, values [nnz] fp32, ids [nnz] int64[, address [nnz] int64]), Faiss's CSR form:
+        query q's matches are [lims[q], lims[q + 1]), by score descending, then address ascending.
+
+        An item matches when search's score for it (the same value, bit for bit) is > threshold, strictly, in fp32; a
+        NaN score never matches.  For euclidean the score is -|x - b|^2 (in search's arithmetic), so Faiss's
+        ``distance < r^2`` is ``threshold = -r^2``.  More than `max_results` matches raise ValueError (naming the
+        total) and return nothing.  Unlike search, this synchronises the stream once, to read the number of matches.
+        """
+        assert x.dim() == 2 and x.shape[0] == self.d_vector
+        assert x.dtype == torch.float32 and x.device == self._storage.device
+        assert x.device.type == "cuda", "torchpq_b200 has no CPU path: the index must live on a CUDA device"
+        t = _range.threshold_f32(threshold)
+        x = x.contiguous()
+        dev, nq, n = x.device, x.shape[1], self._n_items
+        if nq == 0:
+            return _range.empty(0, dev, return_address)
+        norms = self._norm_table() if self.distance != "inner" else None
+        ws_bytes = lib.tpq_flat_range_workspace_bytes(self.d_vector, nq, n)
+        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
+
+        def run(keys, query, cap, total):
+            check(lib.tpq_flat_range_search(ptr(x), self.d_vector, nq, ptr(self._storage), self.capacity, n, ptr(norms),
+                                            _lib.METRIC[self.distance], t, ptr(keys), ptr(query), cap, ptr(total),
+                                            ptr(ws), ws_bytes, _lib.current_stream(dev)))
+        return _range.collect(run, nq, max_results, self._address2id, return_address, dev)

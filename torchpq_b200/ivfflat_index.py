@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib
+from . import _lib, _range
 from ._lib import lib, check, ptr
 from .modules import Codec, IdContainer, _fingerprint
 
@@ -168,6 +168,42 @@ class IVFFlatIndex(IdContainer):
         int64[, address]).  Probes as IVFPQIndex.search (n_probe, use_smart_probing, smart_probing_temperature)."""
         x = self._check_query(x, k)
         return self._search(x, k, int(self.n_probe), None, None, return_address)
+
+    def range_search(self, x, threshold, return_address=False, max_results=1 << 26):
+        """Every item that search would score for a query with a score above `threshold`: x [d_vector, n_query] fp32 on
+        the index device, threshold a float or a 0-d tensor (rounded once to fp32; NaN raises ValueError)
+        -> (lims [n_query + 1] int64, values [nnz] fp32, ids [nnz] int64[, address [nnz] int64]), Faiss's CSR form:
+        query q's matches are [lims[q], lims[q + 1]), by score descending, then address ascending.
+
+        The scored items are search's: the live slots of the cells the query visits under n_probe, use_smart_probing
+        and smart_probing_temperature; holes left by remove never match.  An item matches when its score (search's
+        value, bit for bit) is > threshold, strictly, in fp32; a NaN score never matches.  For euclidean the score is
+        -|x - b|^2 (in search's arithmetic), so Faiss's ``distance < r^2`` is ``threshold = -r^2``.  More than
+        `max_results` matches raise ValueError (naming the total) and return nothing.  Unlike search, this
+        synchronises the stream once, to read the number of matches.
+        """
+        x = self._check_query(x, 1)
+        t = _range.threshold_f32(threshold)
+        dev, nq, n_probe = x.device, x.shape[1], int(self.n_probe)
+        if nq == 0:
+            return _range.empty(0, dev, return_address)
+        assert self.vq_codec.is_trained, "index is not trained"
+        norms = self._norm_table()
+        ws_bytes = lib.tpq_ivfflat_range_workspace_bytes(self.d_vector, nq, self.n_cells, n_probe)
+        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
+        entry, store = self._range_entry()
+
+        def run(keys, query, cap, total):
+            check(entry(ptr(x), self.d_vector, nq, ptr(self.vq_codec.kmeans.centroids), self.n_cells, *store,
+                        self.capacity, ptr(self._is_empty), ptr(self._cell_start), ptr(self._cell_size), ptr(norms),
+                        _lib.METRIC[self.distance], None, None, n_probe, int(bool(self.use_smart_probing)),
+                        float(self.smart_probing_temperature), t, ptr(keys), ptr(query), cap, ptr(total), ptr(ws),
+                        ws_bytes, _lib.current_stream(dev)))
+        return _range.collect(run, nq, max_results, self._address2id, return_address, dev)
+
+    def _range_entry(self):
+        """(the library's range search entry point, its store arguments between n_cells and capacity)."""
+        return lib.tpq_ivfflat_range_search, (ptr(self._storage),)
 
     def search_cells(self, x, cells, n_probe_list=None, k=1, return_address=False):
         """As IVFPQIndex.search_cells: cells [n_query, n_probe] int64 probe lists, n_probe_list [n_query] int64

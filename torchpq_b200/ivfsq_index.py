@@ -127,3 +127,8 @@ class IVFSQIndex(IVFFlatIndex):
         lo, rg = self.sq_codec._bounds(self._storage.device)               # None for 16 bits
         self._sq_bounds = (lo, rg)                                       # kept alive past the launch
         return lib.tpq_ivfsq_search, (ptr(self._storage), self.bits, ptr(lo), ptr(rg))
+
+    def _range_entry(self):
+        lo, rg = self.sq_codec._bounds(self._storage.device)
+        self._sq_bounds = (lo, rg)
+        return lib.tpq_ivfsq_range_search, (ptr(self._storage), self.bits, ptr(lo), ptr(rg))
