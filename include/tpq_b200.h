@@ -217,7 +217,7 @@ int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* vq_codebook,
                      float temperature, int k, const int64_t* address2id, float* values, int64_t* ids,
                      int64_t* address, void* ws, size_t ws_bytes, void* stream);
 
-/* ------------------------------------------------------------------ range search (FlatIndex, IVFFlatIndex, IVFSQIndex)
+/* ------------------------------------------------------------------ range search (FlatIndex, IVFFlatIndex, IVFSQIndex, IVFPQIndex)
  * Every scored item whose score is above the threshold: the same items and scores as the searches above (tpq_flat_search's
  * columns [0, n); the IVF searches' live slots of the visited cells), matched when score > threshold, strictly, in fp32
  * (a NaN score never matches; +-inf thresholds are allowed, a NaN threshold is TPQ_ERR_BAD_ARG).
@@ -235,7 +235,15 @@ int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* vq_codebook,
  *   visiting rule, metrics EUCLIDEAN and COSINE.  A cell is visited at most once per query when cells == NULL (the
  *   coarse probe returns distinct cells).  ws: at least tpq_ivfflat_range_workspace_bytes(d, nq, n_cells, n_probe)
  *   bytes, which stops growing with nq past one chunk of queries (the most whose gathered pair queries, n_probe * d
- *   floats each, fit 256 MB, at most 16 384). */
+ *   floats each, fit 256 MB, at most 16 384).
+ * tpq_ivfpq_range_search: over the IVFPQ scan of tpq_ivfpq_search (cells == NULL: its coarse stage runs inside, with
+ *   cosine normalisation and smart probing, and a cell is visited at most once per query) or of tpq_ivfpq_search_cells
+ *   (cells / n_probe_list given, smart and temperature unused; base_sims [nq, n_probe] required for a residual index).
+ *   The scored items and their scores are those searches', bit for bit: the live slots of the visited cells, ADC sums in
+ *   the scan's order (plus the cell's coarse similarity for a residual index).  On a cell shard (shard_world > 1) only
+ *   the shard's cells are scanned, with global addresses.  Metrics EUCLIDEAN and COSINE (residual: EUCLIDEAN); an index
+ *   without blocks (n_blocks == 0) sets *total = 0.  ws: at least tpq_ivfpq_range_workspace_bytes(index, nq, n_probe)
+ *   bytes. */
 size_t tpq_flat_range_workspace_bytes(int d, int nq, int64_t n);
 int tpq_flat_range_search(const float* x_dn, int d, int nq, const float* base, int64_t ld, int64_t n,
                           const float* norms, int metric, float threshold, uint64_t* match_keys, int32_t* match_query,
@@ -254,6 +262,11 @@ int tpq_ivfsq_range_search(const float* x_dn, int d, int nq, const float* vq_cod
                            int n_probe, int smart, float temperature, float threshold, uint64_t* match_keys,
                            int32_t* match_query, int64_t cap, uint64_t* total, void* ws, size_t ws_bytes,
                            void* stream);
+size_t tpq_ivfpq_range_workspace_bytes(const tpq_index* index, int nq, int n_probe);
+int tpq_ivfpq_range_search(const tpq_index* index, const float* x_dn, const int64_t* cells, const float* base_sims,
+                           const int64_t* n_probe_list, int nq, int n_probe, int smart, float temperature,
+                           float threshold, uint64_t* match_keys, int32_t* match_query, int64_t cap,
+                           uint64_t* total, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------ row-wise top-k (fn.Topk, fn/Topk.py:43-67)
  * x [m, n] row-major, contiguous, fp32 or fp16 (dtype TPQ_DTYPE_*) -> the k best entries of every row: values [m, k]

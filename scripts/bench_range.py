@@ -2,7 +2,8 @@
 
 Workloads (bench.py's generators, as scripts/bench_ivfflat.py):
   * "1M":  1 M x 128 fp32 randn in a FlatIndex (every query scores every vector);
-  * "C3c": the clustered 10 M x 128 C3 set in an IVFFlatIndex, 4096 cells, n_probe 32, smart probing off.
+  * "C3c": the clustered 10 M x 128 C3 set in an IVFFlatIndex, 4096 cells, n_probe 32, smart probing off;
+  * "C3c-pq" / "C3c-res": the same set in an IVFPQIndex with M = 64 (search runs cell-major there), plain / residual.
 nq = 10 000.  Thresholds: for r in {10, 100, 1000}, the median over the queries of search(k = r)'s r-th value, so a
 query gets about r results.
 
@@ -12,14 +13,16 @@ Reported, one JSON line per (workload, r):
     (medians of --steps);
   - flop = 2 d * (vectors scored) and bytes = 4 d * (store vectors read) + 16 B per match (written, then sorted), the
     FP32 compute bound at 67 TFLOP/s and the memory bound at 3.35 TB/s (H100 SXM data sheet), and the share of the
-    larger one that range_search reached;
+    larger one that range_search reached.  IVFPQ: bytes = M * (vectors scanned, summed over the queries) + 12 B per
+    match (the key and the query written by the kernel), against the memory bound;
   - rerun_ms: the same range_search with the first match buffer lowered to 256 entries per query, which forces the one
     re-run (the total is then known exactly and the second pass writes every match).
 --profile: one torch.profiler run per workload at r = 100, kernel time split into the match kernel, the ordering (the
-sorts and the CSR assembly) and the copy of the count.  The card's name, power limit and max SM clock are read in the
+sorts and the CSR assembly) and the copy of the count; IVFPQ adds the range kernel's own CUDA-event time
+(tpq_profile_scan_ms) and its share of the memory bound.  The card's name, power limit and max SM clock are read in the
 same run.
 
-    python scripts/bench_range.py [--workloads 1M,C3c] [--steps 5] [--warmup 2] [--profile] [--out FILE]
+    python scripts/bench_range.py [--workloads 1M,C3c,C3c-pq,C3c-res] [--steps 5] [--warmup 2] [--profile] [--out FILE]
 """
 from __future__ import annotations
 
@@ -57,7 +60,7 @@ def profile_split(fn):
             key = "match_kernel"
         elif "Memcpy DtoH" in n or "Memcpy Device -> Host" in n or "DtoH" in n:
             key = "count_copy"
-        elif "probe" in n or "pairs" in n or "plan_kernel" in n or "gather_kernel" in n or "norm" in n or "Memset" in n \
+        elif "probe" in n or "pairs" in n or "plan_kernel" in n or "gather_kernel" in n or "norm" in n or "coarse" in n or "Memset" in n \
                 or "Memcpy DtoD" in n or "Memcpy Device -> Device" in n or "col_" in n:
             key = "other"
         else:
@@ -67,6 +70,22 @@ def profile_split(fn):
         names[short] = names.get(short, 0.0) + ms
     return {k: round(v, 3) for k, v in split.items()}, \
         {k: round(v, 3) for k, v in sorted(names.items(), key=lambda kv: -kv[1])[:12]}
+
+
+def scan_event_ms(fn, steps):
+    """Median over `steps` calls of fn of the summed CUDA-event time of its scan-kernel launches (tpq_profile_*)."""
+    import ctypes as C
+    import torchpq_b200 as T
+    L = T._lib.lib
+    out = []
+    for _ in range(steps):
+        L.tpq_profile_enable(1)
+        fn()
+        ms, n = C.c_float(), C.c_int()
+        T._lib.check(L.tpq_profile_scan_ms(C.byref(ms), C.byref(n)))
+        L.tpq_profile_enable(0)
+        out.append(ms.value)
+    return sorted(out)[len(out) // 2]
 
 
 def main():
@@ -86,8 +105,16 @@ def main():
     print(json.dumps(lines[-1]), flush=True)
     for wname in args.workloads.split(","):
         t0 = time.time()
-        d, n, C, base, x = workload(wname, dev)
-        if wname == "1M":
+        pq = wname in ("C3c-pq", "C3c-res")
+        d, n, C, base, x = workload("C3c" if pq else wname, dev)
+        M = 64
+        if pq:
+            ix = T.IVFPQIndex(d, M, C, device=str(dev), pq_use_residual=wname == "C3c-res")
+            ix.train(base[:, :1 << 20], seed=0)
+            ix.add(base)
+            ix.n_probe, ix.use_smart_probing = 32, False
+            scored, store = scanned(ix, x, 32, False)
+        elif wname == "1M":
             ix = T.FlatIndex(d, initial_size=n, device=str(dev))
             ix.add(base)
             scored, store = n * x.shape[1], n
@@ -110,7 +137,10 @@ def main():
             nnz = int(lims[-1])
             ms_range, ms_search = alternated_ms([lambda: ix.range_search(x, t), lambda: ix.search(x, k=k)],
                                                 args.steps, args.warmup)
-            flop, byt = 2 * d * scored, 4 * d * store + 16 * nnz
+            if pq:                                   # ADC lookups: no FP32 GEMM; every scanned code is read once
+                flop, byt = 0, M * scored + 12 * nnz
+            else:
+                flop, byt = 2 * d * scored, 4 * d * store + 16 * nnz
             bound_ms = max(flop / PEAK_FP32, byt / PEAK_HBM) * 1e3
             first = _range._FIRST_CAP_PER_QUERY
             _range._FIRST_CAP_PER_QUERY = 256
@@ -129,6 +159,10 @@ def main():
             if args.profile and r == 100:
                 split, top = profile_split(lambda: ix.range_search(x, t))
                 lines.append({"profile": f"{wname} r=100 range_search", "split_ms": split, "kernels_ms": top})
+                if pq:
+                    kern_ms = scan_event_ms(lambda: ix.range_search(x, t), args.steps)
+                    lines[-1].update({"range_kernel_event_ms": round(kern_ms, 3),
+                                      "range_kernel_share_of_hbm": round(M * scored / PEAK_HBM * 1e3 / kern_ms, 4)})
                 print(json.dumps(lines[-1]), flush=True)
                 split, top = profile_split(lambda: ix.search(x, k=100))
                 lines.append({"profile": f"{wname} search k=100", "kernels_ms": top})

@@ -99,6 +99,8 @@ SIGNATURES = {
                                       _P, _I64, _P, _P, _SZ, _P]),
     "tpq_ivfsq_range_search": (_I, [_P, _I, _I, _P, _I, _P, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P, _P, _I, _I, _F,
                                     _F, _P, _P, _I64, _P, _P, _SZ, _P]),
+    "tpq_ivfpq_range_workspace_bytes": (_SZ, [_IX, _I, _I]),
+    "tpq_ivfpq_range_search": (_I, [_IX, _P, _P, _P, _P, _I, _I, _I, _F, _F, _P, _P, _I64, _P, _P, _SZ, _P]),
 }
 
 DTYPE_F32, DTYPE_F16 = 0, 1     # TPQ_DTYPE_* (include/tpq_b200.h)

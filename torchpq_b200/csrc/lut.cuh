@@ -36,8 +36,8 @@ __device__ __forceinline__ float lut_entry(int kind, float dot, float a2, float 
 
 // The LUT of query q in scan layout (RES: the query half of the residual LUT), built by the NW warps of a CTA.  Lane l
 // owns sub-quantizers m = 32 h + l: reads of the transposed codebook are contiguous across the warp, and so is every
-// store (128 B), in shared or global memory.
-template <int MP, int NW, int DSUB, bool RES>
+// store (128 B), in shared or global memory.  CU: how many codes of the codebook loop are unrolled.
+template <int MP, int NW, int DSUB, bool RES, int CU = (DSUB >= 8 ? 2 : 8)>
 __device__ __forceinline__ void build_lut(float* lutf, const float* __restrict__ x, const float* __restrict__ cbt, int M,
                                           int nq, int q, int metric, int lane, int warp) {
   constexpr int NH = MP / 32;
@@ -55,7 +55,7 @@ __device__ __forceinline__ void build_lut(float* lutf, const float* __restrict__
     }
     a2[h] = s2;
   }
-  #pragma unroll (DSUB >= 8 ? 2 : 8)
+  #pragma unroll CU
   for (int c = warp; c < 256; c += NW) {
     #pragma unroll
     for (int h = 0; h < NH; ++h) {

@@ -1,10 +1,15 @@
-// Range search's match buffer, shared by flat_range_kernel (flat.cu) and ivfflat_range_kernel (ivfflat.cu).
+// Range search's match buffers: the CTA's, shared by flat_range_kernel (flat.cu) and ivfflat_range_kernel (ivfflat.cu),
+// and the warp's, of ivfpq_range_kernel (scan.cu).
 //
 // A range kernel keeps no per-query lists: after each 128-column tile's epilogue every thread holds its scores in
 // registers, and the ones above the threshold are appended to one buffer of the CTA in shared memory as (row of the
 // query tile, make_key(score, address)).  When the buffer cannot take another whole tile, and at the end, the CTA
 // reserves its place in the caller's match arrays with one global atomic and copies the buffer out, coalesced.  The
 // global counter always reaches the exact total; entries at or past `cap` are counted and not written.
+//
+// The IVFPQ scan's CTA serves one query, and its warps take 32-vector blocks from a dynamic cursor, each at its own
+// pace: there a warp stages its own matches (keys only: the query is the CTA's) and flushes them itself, by the same
+// rule, when its buffer cannot take another block and when it runs out of blocks.  No CTA barrier is involved.
 #pragma once
 #include "common.cuh"
 
@@ -64,5 +69,42 @@ __device__ __forceinline__ void range_flush(RangeBuf& b, unsigned long long* __r
   if (threadIdx.x == 0) b.cnt = 0;
 }
 #endif  // __CUDACC__
+
+constexpr int kRangeWarpBuf = 96;     // keys a warp stages: it flushes when fewer than a block's 32 places are left
+
+// Where a warp's matches go: a kernel parameter (__grid_constant__, so the warps read it in place, not from registers).
+struct RangeOut {
+  float t;                            // the threshold: a score matches when score > t
+  uint64_t* keys; int32_t* query; int64_t cap; unsigned long long* total;
+};
+
+// One warp's match buffer: buf [kRangeWarpBuf] keys in shared memory, its count in a (warp-uniform) register.
+struct RangeWarpBuf {
+  uint64_t* buf;
+  int cnt;
+  int32_t q;                          // the query every match of the warp belongs to
+  const RangeOut* out;
+#ifdef __CUDACC__
+  // the lanes with `pass` append their keys (every lane calls); flush when another block might not fit
+  __device__ __forceinline__ void push(bool pass, uint64_t key, int lane) {
+    cnt += warp_append(buf, cnt, pass, key, lane);
+    if (cnt > kRangeWarpBuf - 32) flush(lane);
+  }
+  // Lane 0 reserves the run with one global atomic; the lanes copy it out, coalesced.  Ends with the buffer empty.
+  __device__ __forceinline__ void flush(int lane) {
+    if (cnt == 0) return;                              // warp-uniform
+    __syncwarp();                                      // every lane's appended key is visible to the warp
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(out->total, (unsigned long long)cnt);
+    base = __shfl_sync(0xffffffffu, base, 0);
+    for (int i = lane; i < cnt; i += 32) {
+      const unsigned long long g = base + i;
+      if (g < (unsigned long long)out->cap) { out->keys[g] = buf[i]; out->query[g] = q; }
+    }
+    __syncwarp();                                      // every lane has read the buffer before it is refilled
+    cnt = 0;
+  }
+#endif
+};
 
 }  // namespace tpq

@@ -27,6 +27,7 @@
 #include <string.h>
 #include <type_traits>
 #include "lut.cuh"
+#include "range.cuh"
 #include "tc_common.cuh"
 
 namespace tpq {
@@ -82,16 +83,22 @@ __device__ __forceinline__ void adc_unit(const uint32_t (&w)[16], const uint32_t
   }
 }
 
-// This lane's key of a block: the four partial sums of adc_unit are added in this association, on top of `base`, and the
-// lane's address is addr0 + lane.  Every key of both scan kernels is formed here, which is what makes the cell-major
-// path's results the query-major kernel's bit for bit.
+// This lane's score of a block: the four partial sums of adc_unit are added in this association, on top of `base`.
+__device__ __forceinline__ float block_score(const float (&acc)[4], float base) {
+  return base + ((acc[0] + acc[1]) + (acc[2] + acc[3]));
+}
+// This lane's key of a block, its address addr0 + lane.  Every key and every range match of the scan kernels is formed
+// from block_score, which is what makes the cell-major path's results, and range search's scores, the query-major
+// kernel's bit for bit.
 __device__ __forceinline__ uint64_t block_key(const float (&acc)[4], float base, uint32_t addr0, int lane) {
-  return make_key(base + ((acc[0] + acc[1]) + (acc[2] + acc[3])), addr0 + lane);
+  return make_key(block_score(acc, base), addr0 + lane);
 }
 
 // Per-warp scan state.  regs[2][16] is the ping-pong pair of unit buffers; every index into it is a
 // compile-time constant after unrolling (PAR / SB are template parameters), so it lives in registers.
-template <int MP, int NW>
+// RANGE: the blocks' scores go to the warp's range buffer `rs` (every live score above its threshold) instead of the
+// CTA's top-k `tk`.
+template <int MP, int NW, bool RANGE = false>
 struct Scanner {
   static constexpr int NSB = Units<MP>::NSB;
   const uint8_t* codes; const uint32_t* valid; const uint8_t* lut;
@@ -102,7 +109,8 @@ struct Scanner {
   uint32_t regs[2][16];
   CtaTopK tk;
   uint64_t thr;
-  float base;                                           // residual IVFPQ: coarse similarity of the current cell (else 0)
+  RangeWarpBuf rs;
+  float base;                                          // residual IVFPQ: coarse similarity of the current cell (else 0)
   int seg, seg_lo, seg_hi, seg_b0; uint32_t seg_a0;     // current probe segment, cached in registers
   int64_t B_cur, B_nxt; uint32_t a0_cur, a0_nxt, valid_cur, valid_nxt;
 
@@ -131,10 +139,16 @@ struct Scanner {
   __device__ __forceinline__ void process_block(bool has_next) {
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     step<PAR, 0>(acc, has_next);
-    const uint64_t key = block_key(acc, base, a0_cur, lane);
-    const bool live = (valid_cur >> lane) & 1u;
-    if (PAR == 0) thr = tk.threshold();                  // running k-th best of the CTA
-    tk.push(live && key > thr, key, lane);
+    if constexpr (RANGE) {
+      const float s = block_score(acc, base);              // fp32 compare: +0 > -0 is false, a NaN never matches
+      const bool live = (valid_cur >> lane) & 1u;
+      rs.push(live && s > rs.out->t, make_key(s, a0_cur + lane), lane);
+    } else {
+      const uint64_t key = block_key(acc, base, a0_cur, lane);
+      const bool live = (valid_cur >> lane) & 1u;
+      if (PAR == 0) thr = tk.threshold();                // running k-th best of the CTA
+      tk.push(live && key > thr, key, lane);
+    }
     B_cur = B_nxt; a0_cur = a0_nxt; valid_cur = valid_nxt;
   }
   template <int SB>
@@ -243,32 +257,17 @@ __device__ __forceinline__ void write_keys(const ScanArgs& A, const uint64_t* li
   for (int i = tid; i < A.k; i += NW * 32) out[i] = list[i];
 }
 
-// DSUB > 0: the CTA builds its query's LUT itself (build_lut, lut.cuh) from the (L2-resident) transposed codebook -- no
-// LUT round trip through HBM, no LUT workspace.  DSUB == 0: the LUT was staged by lut_kernel (lut.cu) and is copied in.
-// RES: residual IVFPQ (ivfpq_topk_residual_precomputed, ivfpq_topk.cu:1039-1207).  The LUT of a (query, cell) pair
-// is part1[query] + part2[cell]: the query half is built once into a second shared-memory table, and the CTA
-// walks the probed cells in lock step, re-forming the LUT (one float4 add per 16 bytes) before each cell; the
-// cell's coarse similarity seeds every score.
-template <int MP, int NW, int MINB, int DSUB, bool RES>
-__global__ void __launch_bounds__(NW * 32, MINB)
-ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+// The start of a query-major CTA, before its first barrier: warp 0 lays out the query's probe segments (their dependent
+// global loads overlap the other warps' LUT work; visiting rule: probe_entry, scan_layout.cuh) while the CTA stages or
+// builds the LUT (CU: build_lut's unroll).  Returns P, the probe entries the query visits.
+template <int MP, int NW, int DSUB, bool RES, int CU = (DSUB >= 8 ? 2 : 8)>
+__device__ __forceinline__ int scan_prologue(const ScanArgs& A, const ScanSmem& L, uint8_t* smem, int qi, int q, int tid,
+                                             int lane, int warp) {
+  constexpr int MG = lut_groups(MP);
   uint8_t* lut = smem;                                       // L.lut == 0 by construction
   int32_t*  seg_blk0   = reinterpret_cast<int32_t*>(smem + L.seg_blk0);
   uint32_t* seg_addr0  = reinterpret_cast<uint32_t*>(smem + L.seg_addr0);
   int32_t*  seg_prefix = reinterpret_cast<int32_t*>(smem + L.seg_prefix);
-  constexpr int MG = lut_groups(MP);
-
-  const int qi = blockIdx.x / A.S, slice = blockIdx.x % A.S;  // query within this chunk
-  const int q = A.q_base + qi;
-  if (A.only_cnt && A.only_cnt[qi] <= A.only_cap) return;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#ifdef TPQ_DEBUG_KNOBS
-  long long t_ph = clock64();
-#endif
-
-  // --- probe segments first (warp 0): their dependent global loads overlap the other warps' LUT work (visiting rule:
-  // probe_entry, scan_layout.cuh)
   const int P = probe_count<RES>(A.n_probe_list[q], A.n_probe);
   int32_t* seg_cell = reinterpret_cast<int32_t*>(smem + L.seg_cell);
   if (warp == 0) {
@@ -300,9 +299,66 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
     for (int i = tid; i < MG * kLutGroup / 4; i += NW * 32) dst[i] = __ldg(src + i);
   } else {
     // --- build the LUT in place (or, RES, the query half of the residual LUT)
-    build_lut<MP, NW, DSUB, RES>(reinterpret_cast<float*>(RES ? smem + L.part1 : lut), A.x, A.cbt, A.M, A.nq, q, A.metric,
-                                 lane, warp);
+    build_lut<MP, NW, DSUB, RES, CU>(reinterpret_cast<float*>(RES ? smem + L.part1 : lut), A.x, A.cbt, A.M, A.nq, q,
+                                     A.metric, lane, warp);
   }
+  return P;
+}
+
+// Residual IVFPQ's scan of blocks [b_begin, b_end): the CTA walks the visited cells in lock step, re-forms the LUT as
+// part1 + part2 of the cell, seeds every score with the cell's coarse similarity, and runs the Scanner over the cell's
+// blocks.  Called by every thread after the prologue's barrier.
+template <int MP, int NW, int DSUB, class Sc>
+__device__ __forceinline__ void residual_walk(Sc& sc, const ScanArgs& A, const ScanSmem& L, uint8_t* smem, int P,
+                                              int b_begin, int b_end, int q, int qi, int tid) {
+  constexpr int MG = lut_groups(MP);
+  const int32_t* seg_prefix = reinterpret_cast<const int32_t*>(smem + L.seg_prefix);
+  const int32_t* seg_cell = reinterpret_cast<const int32_t*>(smem + L.seg_cell);
+  // query half of the LUT: the shared-memory table built by the prologue (DSUB > 0), or the staged copy in global memory
+  const float4* p1 = DSUB > 0 ? reinterpret_cast<const float4*>(smem + L.part1)
+                              : reinterpret_cast<const float4*>(A.lut_scan + (size_t)qi * MG * kLutGroup);
+  float4* dst = reinterpret_cast<float4*>(smem);
+  for (int j = 0; j < P; ++j) {
+    const int b0 = max(seg_prefix[j], b_begin), b1 = min(seg_prefix[j + 1], b_end);
+    if (b1 <= b0) continue;                                          // skipped entry, empty cell, another shard's or slice's blocks
+    __syncthreads();                                                 // every warp is done with the previous cell's LUT
+    if (tid == 0) *sc.next = b0;
+    const float4* p2 = reinterpret_cast<const float4*>(A.part2_scan + (size_t)seg_cell[j] * MG * kLutGroup);
+    #pragma unroll 4
+    for (int i = tid; i < MG * kLutGroup / 4; i += NW * 32) {                 // store_precomputed_to_smem: part1 + part2 (:609-628)
+      const float4 a = DSUB > 0 ? p1[i] : __ldg(p1 + i), b = __ldg(p2 + i);
+      dst[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    }
+    __syncthreads();
+    sc.base = A.base_sims[(size_t)q * A.n_probe + j];
+    sc.run(b1);
+  }
+}
+
+// DSUB > 0: the CTA builds its query's LUT itself (build_lut, lut.cuh) from the (L2-resident) transposed codebook -- no
+// LUT round trip through HBM, no LUT workspace.  DSUB == 0: the LUT was staged by lut_kernel (lut.cu) and is copied in.
+// RES: residual IVFPQ (ivfpq_topk_residual_precomputed, ivfpq_topk.cu:1039-1207).  The LUT of a (query, cell) pair
+// is part1[query] + part2[cell]: the query half is built once into a second shared-memory table, and the CTA
+// walks the probed cells in lock step, re-forming the LUT (one float4 add per 16 bytes) before each cell; the
+// cell's coarse similarity seeds every score.
+template <int MP, int NW, int MINB, int DSUB, bool RES>
+__global__ void __launch_bounds__(NW * 32, MINB)
+ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* lut = smem;                                       // L.lut == 0 by construction
+  int32_t*  seg_blk0   = reinterpret_cast<int32_t*>(smem + L.seg_blk0);
+  uint32_t* seg_addr0  = reinterpret_cast<uint32_t*>(smem + L.seg_addr0);
+  int32_t*  seg_prefix = reinterpret_cast<int32_t*>(smem + L.seg_prefix);
+
+  const int qi = blockIdx.x / A.S, slice = blockIdx.x % A.S;  // query within this chunk
+  const int q = A.q_base + qi;
+  if (A.only_cnt && A.only_cnt[qi] <= A.only_cap) return;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#ifdef TPQ_DEBUG_KNOBS
+  long long t_ph = clock64();
+#endif
+
+  const int P = scan_prologue<MP, NW, DSUB, RES>(A, L, smem, qi, q, tid, lane, warp);
 #ifdef TPQ_DEBUG_KNOBS
   auto phase_mark = [&](int i) {
     if (A.phase && tid == 0) { const long long t = clock64(); atomicAdd(A.phase + i, (unsigned long long)(t - t_ph)); t_ph = t; }
@@ -327,25 +383,7 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
   sc.seg = 0; sc.seg_lo = 0; sc.seg_hi = seg_prefix[1]; sc.seg_b0 = seg_blk0[0]; sc.seg_a0 = seg_addr0[0];
   CtaTopK& tk = sc.tk;
   if constexpr (RES) {
-    // query half of the LUT: the shared-memory table built above (DSUB > 0), or the staged copy in global memory
-    const float4* p1 = DSUB > 0 ? reinterpret_cast<const float4*>(smem + L.part1)
-                                : reinterpret_cast<const float4*>(A.lut_scan + (size_t)qi * MG * kLutGroup);
-    float4* dst = reinterpret_cast<float4*>(lut);
-    for (int j = 0; j < P; ++j) {
-      const int b0 = max(seg_prefix[j], b_begin), b1 = min(seg_prefix[j + 1], b_end);
-      if (b1 <= b0) continue;                                          // skipped entry, empty cell, another shard's or slice's blocks
-      __syncthreads();                                                 // every warp is done with the previous cell's LUT
-      if (tid == 0) *sc.next = b0;
-      const float4* p2 = reinterpret_cast<const float4*>(A.part2_scan + (size_t)seg_cell[j] * MG * kLutGroup);
-      #pragma unroll 4
-      for (int i = tid; i < MG * kLutGroup / 4; i += NW * 32) {                 // store_precomputed_to_smem: part1 + part2 (:609-628)
-        const float4 a = DSUB > 0 ? p1[i] : __ldg(p1 + i), b = __ldg(p2 + i);
-        dst[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-      }
-      __syncthreads();
-      sc.base = A.base_sims[(size_t)q * A.n_probe + j];
-      sc.run(b1);
-    }
+    residual_walk<MP, NW, DSUB>(sc, A, L, smem, P, b_begin, b_end, q, qi, tid);
     tk.cta_drain(lane, warp);
     write_keys<NW>(A, tk.list, q, slice, tid);
     return;
@@ -377,6 +415,48 @@ ivfpq_scan_kernel(ScanArgs A, ScanSmem L) {
 #endif
   write_keys<NW>(A, tk.list, q, slice, tid);
 }
+#undef TPQ_PHASE
+
+// The range search's query-major kernel: ivfpq_scan_kernel's CTA per (query, slice), its prologue, residual walk and
+// Scanner, with every live score above R.t kept instead of a top-k.  Each warp stages its matches in its own
+// kRangeWarpBuf keys (range.cuh), in the shared memory the top-k of a k = 1 search takes (scan_smem's topk), and
+// flushes them itself.
+template <int MP, int NW, int MINB, int DSUB, bool RES>
+__global__ void __launch_bounds__(NW * 32, MINB)
+ivfpq_range_kernel(ScanArgs A, ScanSmem L, const __grid_constant__ RangeOut R) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  static_assert((size_t)NW * kRangeWarpBuf * 8 <= CtaTopK::bytes(NW, 32), "a warp's range buffer lies in the k = 1 top-k's place");
+  const int qi = blockIdx.x / A.S, slice = blockIdx.x % A.S;
+  const int q = A.q_base + qi;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int32_t* seg_blk0 = reinterpret_cast<int32_t*>(smem + L.seg_blk0);
+  uint32_t* seg_addr0 = reinterpret_cast<uint32_t*>(smem + L.seg_addr0);
+  int32_t* seg_prefix = reinterpret_cast<int32_t*>(smem + L.seg_prefix);
+  // the LUT build of ivfpq_scan_kernel<192, 16, 1, 4, false> spills; here its codebook loop is unrolled 4 times, not 8
+  constexpr int CU = (MP == 192 && DSUB == 4) ? 4 : (DSUB >= 8 ? 2 : 8);
+  const int P = scan_prologue<MP, NW, DSUB, RES, CU>(A, L, smem, qi, q, tid, lane, warp);
+  Scanner<MP, NW, true> sc;
+  sc.codes = A.codes; sc.valid = A.valid; sc.lut = smem;
+  sc.seg_prefix = seg_prefix; sc.seg_blk0 = seg_blk0; sc.seg_addr0 = seg_addr0; sc.lane = lane;
+  sc.next = reinterpret_cast<int*>(smem + L.next);
+  sc.rs = RangeWarpBuf{reinterpret_cast<uint64_t*>(smem + L.topk) + (size_t)warp * kRangeWarpBuf, 0, q, &R};
+  lane_slot_offsets(sc.off, lane);
+  __syncthreads();
+  const int total = seg_prefix[P];
+  const int b_begin = (int)(((int64_t)total * slice) / A.S);
+  const int b_end = (int)(((int64_t)total * (slice + 1)) / A.S);
+  sc.base = 0.f;
+  sc.seg = 0; sc.seg_lo = 0; sc.seg_hi = seg_prefix[1]; sc.seg_b0 = seg_blk0[0]; sc.seg_a0 = seg_addr0[0];
+  if constexpr (RES) {
+    residual_walk<MP, NW, DSUB>(sc, A, L, smem, P, b_begin, b_end, q, qi, tid);
+  } else {
+    if (tid == 0) *sc.next = b_begin;
+    __syncthreads();
+    sc.run(b_end);
+  }
+  sc.rs.flush(lane);                                       // what is left when the warp runs out of blocks
+}
+
 
 // ----------------------------------------------------------------------------- merge + decode
 // keys_in: n_parts sorted lists of k keys per query -> top-k, decoded.
@@ -840,7 +920,8 @@ struct SearchWs {
 // the three search entry points all read the plan.
 struct ScanPlan {
   int S, chunk;                   // CTAs (slices) per query; queries per scan launch
-  bool cell_major;                // the cell-major stage (ivfpq_cell_scan_kernel) instead of one query-major launch
+  bool range;                     // range search: ivfpq_range_kernel, no keys workspace, never cell-major
+  bool cell_major;               // the cell-major stage (ivfpq_cell_scan_kernel) instead of one query-major launch
   int dsub;                       // LUT source: d/M = 1, 2, 4 or 8 when built in the kernel (on the cell-major path:
                                   // by cell_lut_kernel), 0 = staged through global memory by lut_kernel
   bool residual, part1_in_smem;   // residual IVFPQ; its query half of the LUT in a second shared-memory table
@@ -868,7 +949,7 @@ static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, const
   w.npl = off;        off += align_up((size_t)nq * 8, 256);
   w.xnorm = off;      off += align_up((size_t)nq * ix->d_vector * 4, 256);
   w.lut = off;        off += P.qm_dsub() ? 0 : align_up((size_t)P.chunk * lut_bytes(ix->m_pad), 256);
-  w.keys = off;       off += align_up((size_t)nq * P.S * k * 8, 256);
+  w.keys = off;       off += P.range ? 0 : align_up((size_t)nq * P.S * k * 8, 256);
   const size_t C = cm ? (size_t)ix->n_cells : 0, pairs = cm ? (size_t)P.chunk * n_probe : 0;
   const size_t n_items = cm ? C + (size_t)ix->n_blocks / (P.cell_nw * P.cell_r) + 1 : 0;
   w.cell_cnt = off;   off += align_up((C + 2) * 4, 256);                  // pairs per cell, then the item count and cursor
@@ -885,9 +966,12 @@ static SearchWs search_ws(const tpq_index* ix, int nq, int n_probe, int k, const
   return w;
 }
 
-// push: the fused-push path (tpq_ivfpq_scan_push), which keeps the query-major kernel
-static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool push) {
+// push: the fused-push path (tpq_ivfpq_scan_push), which keeps the query-major kernel.  range: range search
+// (tpq_ivfpq_range_search, k = 1), the query-major kernel's slicing, chunking and configuration with
+// ivfpq_range_kernel in its place; its shared memory is that of a k = 1 search.
+static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool push, bool range = false) {
   ScanPlan P{};
+  P.range = range;
   const int dsub = ix->d_vector / ix->n_subvectors;
   const int want = device_sm_count() * 4;       // enough CTAs for ~2 waves of 2 CTAs/SM when the batch is small
   P.S = nq >= want ? 1 : ((want + nq - 1) / nq > 64 ? 64 : (want + nq - 1) / nq);
@@ -947,7 +1031,7 @@ static ScanPlan plan_scan(const tpq_index* ix, int nq, int n_probe, int k, bool 
   // M <= 64, with an in-kernel LUT build, whose cells hold more than kCellMinLive live vectors (codes) on average, on an
   // unsliced batch.  Unsharded only: on a cell shard, a query's entry 0 is usually another shard's cell, which gives
   // pass 1 no vectors and the bound 0, so every owned candidate would survive and overflow.
-  P.cell_major = !push && !P.residual && P.MP == 64 && P.dsub && P.S == 1 && ix->shard_world == 1 && ix->n_blocks > 0 &&
+  P.cell_major = !push && !range && !P.residual && P.MP == 64 && P.dsub && P.S == 1 && ix->shard_world == 1 && ix->n_blocks > 0 &&
                  ix->mean_cell_live >= kCellMinLive;
   if (P.cell_major) { P.NW = 8; P.MINB = 2; }        // pass 1 and the overflow re-run: 120 registers, 0 spill bytes
   P.part1_in_smem = P.residual && P.dsub > 0;
@@ -1010,6 +1094,45 @@ static ScanKernel scan_kernel(const ScanPlan& P) {
     case 4:  return scan_kernel_d<4>(P);
     case 8:  return scan_kernel_d<8>(P);
     default: return scan_kernel_d<0>(P);
+  }
+}
+// The plan's range kernel, scan_kernel's counterpart: one ivfpq_range_kernel for every configuration the product plan
+// picks, and only those (the debug build's other configurations have none: nullptr).
+using RangeKernel = void (*)(ScanArgs, ScanSmem, RangeOut);
+template <int DSUB>
+static RangeKernel range_kernel_d(const ScanPlan& P) {
+  if (P.residual) {
+    if (P.NW != 16) return nullptr;
+    if constexpr (DSUB == 1 || DSUB == 2 || DSUB == 4)
+      return P.MP == 32 ? ivfpq_range_kernel<32, 16, 1, DSUB, true> : ivfpq_range_kernel<64, 16, 1, DSUB, true>;
+    switch (P.MP) {
+      case 32:  return ivfpq_range_kernel<32, 16, 1, 0, true>;
+      case 64:  return ivfpq_range_kernel<64, 16, 1, 0, true>;
+      case 96:  return ivfpq_range_kernel<96, 16, 1, 0, true>;
+      case 128: return ivfpq_range_kernel<128, 16, 1, 0, true>;
+      case 160: return ivfpq_range_kernel<160, 16, 1, 0, true>;
+      case 192: return ivfpq_range_kernel<192, 16, 1, 0, true>;
+    }
+    return nullptr;
+  }
+  if (P.MP <= 64 && P.NW != 8) return nullptr;
+  switch (P.MP) {
+    case 32:  return ivfpq_range_kernel<32, 8, 2, DSUB, false>;
+    case 64:  return P.MINB == 2 ? ivfpq_range_kernel<64, 8, 2, DSUB, false> : ivfpq_range_kernel<64, 8, 3, DSUB, false>;
+    case 96:  return ivfpq_range_kernel<96, 16, 1, DSUB, false>;
+    case 128: return ivfpq_range_kernel<128, 16, 1, DSUB, false>;
+    case 160: return ivfpq_range_kernel<160, 16, 1, DSUB, false>;
+    case 192: return ivfpq_range_kernel<192, 16, 1, DSUB, false>;
+  }
+  return nullptr;
+}
+static RangeKernel range_kernel(const ScanPlan& P) {
+  switch (P.dsub) {                                          // a range plan is never cell-major: qm_dsub() == dsub
+    case 1:  return range_kernel_d<1>(P);
+    case 2:  return range_kernel_d<2>(P);
+    case 4:  return range_kernel_d<4>(P);
+    case 8:  return range_kernel_d<8>(P);
+    default: return range_kernel_d<0>(P);
   }
 }
 using CellLutKernel = decltype(&cell_lut_kernel<1>);
@@ -1115,12 +1238,14 @@ static int cell_stage(const ScanPlan& P, const ScanJob& J, ScanKernel qmajor, Sc
 }
 
 // Every scan launch of a batch, per chunk of P.chunk queries: the cell-major stage, or the staged LUT (when there is
-// one) and the query-major kernel.  The profiling events bracket the scan stage of each chunk: the whole cell-major
-// stage, or the query-major kernel.
-static int launch(const ScanPlan& P, const ScanJob& J) {
+// one) and the query-major kernel -- on a range plan the range kernel, whose matches go to R.  The profiling events
+// bracket the scan stage of each chunk: the whole cell-major stage, or the query-major (or range) kernel.
+static int launch(const ScanPlan& P, const ScanJob& J, const RangeOut* R = nullptr) {
   const tpq_index* ix = J.ix;
-  const ScanKernel kern = scan_kernel(P);
-  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.L.total));
+  const ScanKernel kern = P.range ? nullptr : scan_kernel(P);
+  const RangeKernel rkern = P.range ? range_kernel(P) : nullptr;
+  if (P.range) TPQ_CUDA(cudaFuncSetAttribute(rkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.L.total));
+  else TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.L.total));
   for (int q0 = 0; q0 < J.nq; q0 += P.chunk) {
     const int n = (J.nq - q0) < P.chunk ? (J.nq - q0) : P.chunk;
     if (!P.cell_major && P.dsub == 0) {
@@ -1131,7 +1256,10 @@ static int launch(const ScanPlan& P, const ScanJob& J) {
     const ScanArgs A = scan_args(P, J, q0);
     const bool prof = g_prof_on && g_prof_n < kProfMax;
     if (prof) cudaEventRecord(g_prof_start[g_prof_n], J.st);
-    if (P.cell_major) {
+    if (P.range) {
+      rkern<<<n * P.S, P.NW * 32, P.L.total, J.st>>>(A, P.L, *R);
+      TPQ_LAUNCH_CHECK("ivfpq_range_kernel");
+    } else if (P.cell_major) {
       if (int rc = cell_stage(P, J, kern, A, q0, n)) return rc;
     } else {
       kern<<<n * P.S, P.NW * 32, P.L.total, J.st>>>(A, P.L);
@@ -1282,6 +1410,48 @@ extern "C" int tpq_ivfpq_scan_push(const tpq_index* ix, const float* x_dn, const
   return search(ix, Probes{x_dn, base_sims, cells, n_probe_list}, nq, n_probe, k, smart, temperature,
                 SearchOut{nullptr, nullptr, nullptr, nullptr, peer_keys, n_peers, my_slot}, ws, ws_bytes,
                 (cudaStream_t)stream);
+}
+
+// ----------------------------------------------------------------------------- range search
+extern "C" size_t tpq_ivfpq_range_workspace_bytes(const tpq_index* ix, int nq, int n_probe) {
+  if (!ix || nq <= 0 || n_probe <= 0) return 0;
+  return plan_scan(ix, nq, n_probe, 1, /*push=*/false, /*range=*/true).ws.total;
+}
+
+// cells == nullptr: the coarse stage of tpq_ivfpq_search runs here; else the probe lists of tpq_ivfpq_search_cells
+extern "C" int tpq_ivfpq_range_search(const tpq_index* ix, const float* x_dn, const int64_t* cells, const float* base_sims,
+                                      const int64_t* n_probe_list, int nq, int n_probe, int smart, float temperature,
+                                      float threshold, uint64_t* match_keys, int32_t* match_query, int64_t cap,
+                                      uint64_t* total, void* ws, size_t ws_bytes, void* stream) {
+  if (int rc = check_index(ix, 1)) return rc;
+  TPQ_REQUIRE(nq >= 0 && x_dn, "tpq_ivfpq_range_search: bad query batch");
+  TPQ_REQUIRE((cells == nullptr) == (n_probe_list == nullptr), "tpq_ivfpq_range_search: cells and n_probe_list go together");
+  TPQ_REQUIRE(n_probe >= 1 && (cells || n_probe <= ix->n_cells), "n_probe=%d must be in [1, n_cells=%d]", n_probe, ix->n_cells);
+  if (!cells && n_probe > 1024) { set_error("n_probe=%d > 1024 is not supported", n_probe); return TPQ_ERR_UNSUPPORTED; }
+  TPQ_REQUIRE(threshold == threshold, "tpq_ivfpq_range_search: the threshold is NaN");
+  TPQ_REQUIRE(cap >= 0, "tpq_ivfpq_range_search: cap=%lld is negative", (long long)cap);
+  TPQ_REQUIRE(total && (cap == 0 || (match_keys && match_query)), "tpq_ivfpq_range_search: null total or match buffer");
+  if (ix->residual && (!ix->part2_scan || (cells && !base_sims))) {
+    set_error("tpq_ivfpq_range_search: residual search needs part2_scan and base_sims");
+    return TPQ_ERR_BAD_ARG;
+  }
+  if (nq == 0) return TPQ_OK;
+  const ScanPlan P = plan_scan(ix, nq, n_probe, 1, /*push=*/false, /*range=*/true);
+  if (P.rc) { set_error("%s", P.err); return P.rc; }
+  if (!range_kernel(P)) { set_error("tpq_ivfpq_range_search: no range kernel for this scan configuration"); return TPQ_ERR_UNSUPPORTED; }
+  if (!ws || ws_bytes < P.ws.total) {
+    set_error("tpq_ivfpq_range_search: workspace too small (%zu < %zu)", ws_bytes, P.ws.total);
+    return TPQ_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  TPQ_CUDA(cudaMemsetAsync(total, 0, sizeof(uint64_t), st));
+  if (ix->n_blocks == 0) return TPQ_OK;                     // nothing to score
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  Probes p{x_dn, base_sims, cells, n_probe_list};
+  if (!cells)
+    if (int rc = coarse_stage(ix, x_dn, nq, n_probe, smart, temperature, w, P.ws, st, p)) return rc;
+  const RangeOut R{threshold, match_keys, match_query, cap, reinterpret_cast<unsigned long long*>(total)};
+  return launch(P, ScanJob{ix, p.x, p.cells, p.npl, p.sims, nq, n_probe, 1, w, st, nullptr, 0, 0}, &R);
 }
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k,

@@ -16,7 +16,7 @@ from typing import Optional
 
 import torch
 
-from . import _lib
+from . import _lib, _range
 from ._lib import lib, check, ptr
 from .modules import Codec, IdContainer, _fingerprint
 
@@ -285,6 +285,36 @@ class IVFPQIndex(IdContainer):
         return self._search(x, k, n_probe, lambda ix, *out: lib.tpq_ivfpq_search(ix, ptr(x), x.shape[1], n_probe, k, smart,
                                                                                   temperature, *out),
                             return_address=return_address, return_keys=return_keys)
+
+    def range_search(self, x, threshold, return_address=False, max_results=1 << 26):
+        """Every item that search would score for a query with a score above `threshold`: x [d_vector, n_query] fp32 on
+        the index device, threshold a float or a 0-d tensor (rounded once to fp32; NaN raises ValueError)
+        -> (lims [n_query + 1] int64, values [nnz] fp32, ids [nnz] int64[, address [nnz] int64]), Faiss's CSR form:
+        query q's matches are [lims[q], lims[q + 1]), by score descending, then address ascending.
+
+        The scored items are search's: the live slots of the cells the query visits under n_probe, use_smart_probing
+        and smart_probing_temperature; holes left by remove never match.  An item matches when its score (search's
+        value, bit for bit: the ADC score, plus the cell's coarse similarity for a residual index) is > threshold,
+        strictly, in fp32; a NaN score never matches.  For euclidean the score approximates -|x - b|^2, so Faiss's
+        ``distance < r^2`` is ``threshold = -r^2``.  On a cell shard (set_shard) only the shard's cells are scanned.
+        More than `max_results` matches raise ValueError (naming the total) and return nothing.  Unlike search, this
+        synchronises the stream once, to read the number of matches.
+        """
+        x = self._check_query(x, 1)
+        t = _range.threshold_f32(threshold)
+        dev, nq, n_probe = x.device, x.shape[1], int(self.n_probe)
+        if nq == 0 or self._address2id.shape[0] == 0:                   # no queries, or an index without a slot
+            return _range.empty(nq, dev, return_address)
+        lay = self.layout()
+        smart, temperature = int(bool(self.use_smart_probing)), float(self.smart_probing_temperature)
+        ws_bytes = lib.tpq_ivfpq_range_workspace_bytes(C.byref(lay.cindex), nq, n_probe)
+        ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
+
+        def run(keys, query, cap, total):
+            check(lib.tpq_ivfpq_range_search(C.byref(lay.cindex), ptr(x), None, None, None, nq, n_probe, smart,
+                                             temperature, t, ptr(keys), ptr(query), cap, ptr(total), ptr(ws), ws_bytes,
+                                             _lib.current_stream(dev)))
+        return _range.collect(run, nq, max_results, self._address2id, return_address, dev)
 
     def search_cells(self, x, cells, base_sims=None, n_probe_list=None, k=1, return_address=False, return_keys=False):
         """IVFPQIndex.search_cells, non-residual branch (IVFPQIndex.py:407-467)."""

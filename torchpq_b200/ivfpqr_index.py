@@ -177,6 +177,10 @@ class IVFPQRIndex(IVFPQIndex):
     def search_cells(self, *args, **kwargs):
         raise NotImplementedError("IVFPQRIndex.search_cells is not implemented: use search")
 
+    def range_search(self, *args, **kwargs):
+        # IVFPQIndex.range_search would return the first pass's ADC scores, not the re-ranked ones
+        raise NotImplementedError("IVFPQRIndex.range_search is not implemented: its scores would not be re-ranked")
+
     def scan_push(self, *args, **kwargs):
         raise NotImplementedError("IVFPQRIndex has no fused multi-GPU scan: the re-rank pass reads _storage")
 
