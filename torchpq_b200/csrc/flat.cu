@@ -4,8 +4,7 @@
 // so the [nq, n] score matrix never reaches HBM (10 k queries x 1 M vectors would be 40 GB).  Each CTA owns QT queries
 // and one slice of the base columns; it writes its queries' sorted top-k keys to ws[slice, q, :], and
 // tpq_merge_topk merges the slices and decodes values, addresses and ids.
-#include "gemm_tile.cuh"
-#include "range.cuh"
+#include "fused_scan.cuh"
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k, const int64_t* address2id,
                               int64_t capacity, float* values, int64_t* ids, int64_t* address, void* stream);
@@ -13,15 +12,8 @@ extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int 
 namespace tpq {
 
 constexpr float kFlatEps = 1e-8f;     // metric.cosine_similarity's `norm + 1e-8` (metric.py:14-25)
-constexpr int kFlatWarps = 8;
 
-// Shared memory of one CTA: GEMM stages | score tile [QT][128] f32 | lists [QT][kp] keys | staging [8][kTopkBuf] keys.
-static size_t flat_smem_bytes(int qt, int kp) {
-  const size_t stages = 2 * (size_t)GK * (qt + GB) * 4;
-  return stages + (size_t)qt * GB * 4 + (size_t)qt * kp * 8 + (size_t)kFlatWarps * kTopkBuf * 8;
-}
-
-// The plan, read by the workspace size and the launch.
+// The plan, read by the workspace size and the launch; k == 0 is the range search's, with no lists and no keys.
 //   QT: the smallest of 16, 32, 64 that holds the batch (a 1-query batch does not pay for 64 rows of GEMM), halved
 //       while the CTA's shared memory exceeds 227 KB.  k <= 256 keeps 64 (kp = 256: 24 + 32 + 128 + 4 = 188 KB),
 //       k = 512 gives 32 (20 + 16 + 128 + 4 = 168 KB), k = 1024 gives 16 (18 + 8 + 128 + 4 = 158 KB).  64 is the
@@ -37,11 +29,11 @@ struct FlatPlan {
 
 static FlatPlan plan_flat(int d, int nq, int64_t n, int k) {
   FlatPlan P{};
-  P.kp = list_capacity(k);
+  P.kp = k ? list_capacity(k) : 0;
   P.qt = 16;
   while (P.qt < 64 && P.qt < nq) P.qt *= 2;
-  while (P.qt > 16 && flat_smem_bytes(P.qt, P.kp) > kSmemLimit) P.qt /= 2;
-  P.smem = flat_smem_bytes(P.qt, P.kp);
+  while (P.qt > 16 && fused_smem_bytes(P.qt, P.kp) > kSmemLimit) P.qt /= 2;
+  P.smem = fused_smem_bytes(P.qt, P.kp);
   P.qtiles = (nq + P.qt - 1) / P.qt;
   const int64_t tiles = (n + GB - 1) / GB;
   int64_t S = (2 * (int64_t)device_sm_count() + P.qtiles - 1) / P.qtiles;
@@ -102,7 +94,7 @@ flat_search_kernel(const float* __restrict__ x, int d, int nq, const float* __re
     }
     __syncthreads();
     // warp w owns rows w, w + 8, ...: filter each against its query's k-th key, stage the survivors, flush per row
-    for (int r = warp; r < QT && q0 + r < nq; r += kFlatWarps) {
+    for (int r = warp; r < QT && q0 + r < nq; r += kFusedWarps) {
       WarpTopK tk{lists + (size_t)r * kp, wbuf, kp, k, 0};
       uint64_t thr = tk.kth();
       #pragma unroll
@@ -116,56 +108,10 @@ flat_search_kernel(const float* __restrict__ x, int d, int nq, const float* __re
     }
   }
   __syncthreads();                                     // the lists were last written by their own warps
-  for (int r = warp; r < QT && q0 + r < nq; r += kFlatWarps) {
+  for (int r = warp; r < QT && q0 + r < nq; r += kFusedWarps) {
     uint64_t* dst = keys_out + ((size_t)blockIdx.y * nq + q0 + r) * k;
     for (int i = lane; i < k; i += 32) dst[i] = lists[(size_t)r * kp + i];
   }
-}
-
-template <int QT>
-static int launch_flat(int metric, const FlatPlan& P, const float* x, int d, int nq, const float* base, int64_t ld,
-                       int64_t n, const float* norms, const float* xn, int k, uint64_t* keys, cudaStream_t st) {
-  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? flat_search_kernel<QT, TPQ_METRIC_EUCLIDEAN>
-            : metric == TPQ_METRIC_COSINE    ? flat_search_kernel<QT, TPQ_METRIC_COSINE>
-                                             : flat_search_kernel<QT, TPQ_METRIC_INNER>;
-  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
-  kern<<<dim3(P.qtiles, P.S), 256, P.smem, st>>>(x, d, nq, base, ld, n, norms, xn, k, P.kp, P.slice_cols, keys);
-  TPQ_LAUNCH_CHECK("flat_search_kernel");
-  return TPQ_OK;
-}
-
-static bool flat_metric(int metric) {
-  return metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE || metric == TPQ_METRIC_INNER;
-}
-
-// ----------------------------------------------------------------------------- range search
-// Shared memory of one range CTA: GEMM stages | match buffer (range.cuh).  QT = 64: 24 + 81 = 105 KB, two CTAs per SM.
-static size_t flat_range_smem_bytes(int qt) { return 2 * (size_t)GK * (qt + GB) * 4 + sizeof(RangeBuf); }
-
-// The plan of tpq_flat_range_search: QT and S as plan_flat's (no lists, so QT never halves); the workspace is |x|^2 and
-// the normalised queries.
-struct FlatRangePlan {
-  int qt, qtiles, S;
-  int64_t slice_cols;
-  size_t smem, xn, xq, total;
-};
-
-static FlatRangePlan plan_flat_range(int d, int nq, int64_t n) {
-  FlatRangePlan P{};
-  P.qt = 16;
-  while (P.qt < 64 && P.qt < nq) P.qt *= 2;
-  P.smem = flat_range_smem_bytes(P.qt);
-  P.qtiles = (nq + P.qt - 1) / P.qt;
-  const int64_t tiles = (n + GB - 1) / GB;
-  int64_t S = (2 * (int64_t)device_sm_count() + P.qtiles - 1) / P.qtiles;
-  S = S < 1 ? 1 : (tiles > 0 && S > tiles ? tiles : S);
-  const int64_t per = tiles > 0 ? (tiles + S - 1) / S : 1;
-  P.S = tiles > 0 ? (int)((tiles + per - 1) / per) : 1;
-  P.slice_cols = per * GB;
-  P.xn = 0;
-  P.xq = align_up((size_t)nq * 4, 256);
-  P.total = P.xq + align_up((size_t)d * nq * 4, 256);
-  return P;
 }
 
 // grid (query tiles, slices), 256 threads.  flat_search_kernel's GEMM and epilogue, then every score > thr (strict, in
@@ -220,17 +166,39 @@ flat_range_kernel(const float* __restrict__ x, int d, int nq, const float* __res
   range_flush(mb, total, cap, keys_out, q_out, query);
 }
 
-template <int QT>
-static int launch_flat_range(int metric, const FlatRangePlan& P, const float* x, int d, int nq, const float* base,
-                             int64_t ld, int64_t n, const float* norms, const float* xn, float thr, uint64_t* keys,
-                             int32_t* query, int64_t cap, unsigned long long* total, cudaStream_t st) {
-  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? flat_range_kernel<QT, TPQ_METRIC_EUCLIDEAN>
-            : metric == TPQ_METRIC_COSINE    ? flat_range_kernel<QT, TPQ_METRIC_COSINE>
-                                             : flat_range_kernel<QT, TPQ_METRIC_INNER>;
-  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
-  kern<<<dim3(P.qtiles, P.S), 256, P.smem, st>>>(x, d, nq, base, ld, n, norms, xn, thr, P.slice_cols, keys, query, cap,
-                                                 total);
-  TPQ_LAUNCH_CHECK("flat_range_kernel");
+static bool flat_metric(int metric) {
+  return metric == TPQ_METRIC_EUCLIDEAN || metric == TPQ_METRIC_COSINE || metric == TPQ_METRIC_INNER;
+}
+
+// The checks of tpq_flat_search and tpq_flat_range_search on the sizes.
+static int flat_check(const char* name, int d, int nq, int64_t n, int64_t ld) {
+  TPQ_REQUIRE(d > 0 && nq >= 0 && n >= 0 && ld >= n, "%s: bad sizes d=%d nq=%d n=%lld ld=%lld", name, d, nq,
+              (long long)n, (long long)ld);
+  TPQ_REQUIRE(n < (int64_t(1) << 32), "%s: n=%lld exceeds the 32-bit address of a key", name, (long long)n);
+  return TPQ_OK;
+}
+
+// The rest of both searches up to the launch, for nq > 0: the query, base and norm pointers, the plan P (k == 0: the
+// range search's) and the workspace, then the queries the GEMM reads, xq: x_dn with |x|^2 at P.xn (euclidean), or the
+// normalised queries at P.xq (cosine).  n == 0 reads no query.
+static int flat_prepare(const char* name, const float* x_dn, int d, int nq, const float* base, int64_t n,
+                        const float* norms, int metric, int k, void* ws, size_t ws_bytes, cudaStream_t st,
+                        FlatPlan& P, const float*& xq) {
+  TPQ_REQUIRE(x_dn, "%s: null query pointer", name);
+  TPQ_REQUIRE(n == 0 || (base && (norms || metric == TPQ_METRIC_INNER)), "%s: null base or norms", name);
+  P = plan_flat(d, nq, n, k);
+  if (!ws || ws_bytes < P.total) {
+    set_error("%s: workspace too small (%zu < %zu)", name, ws_bytes, P.total);
+    return TPQ_ERR_WORKSPACE;
+  }
+  xq = x_dn;
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  if (n == 0) return TPQ_OK;
+  if (metric == TPQ_METRIC_EUCLIDEAN) return col_sqnorms(x_dn, d, nq, nq, reinterpret_cast<float*>(w + P.xn), st);
+  if (metric == TPQ_METRIC_COSINE) {
+    xq = reinterpret_cast<float*>(w + P.xq);
+    return normalize_columns(x_dn, d, nq, kFlatEps, reinterpret_cast<float*>(w + P.xq), st);
+  }
   return TPQ_OK;
 }
 
@@ -260,37 +228,20 @@ extern "C" int tpq_flat_search(const float* x_dn, int d, int nq, const float* ba
   TPQ_REQUIRE(k > 0, "k must be in (0, 1024], got %d", k);
   if (k > 1024) { set_error("k=%d > 1024 is not supported", k); return TPQ_ERR_UNSUPPORTED; }
   if (!flat_metric(metric)) { set_error("tpq_flat_search: unsupported metric %d", metric); return TPQ_ERR_UNSUPPORTED; }
-  TPQ_REQUIRE(d > 0 && nq >= 0 && n >= 0 && ld >= n, "tpq_flat_search: bad sizes d=%d nq=%d n=%lld ld=%lld", d, nq,
-              (long long)n, (long long)ld);
-  TPQ_REQUIRE(n < (int64_t(1) << 32), "tpq_flat_search: n=%lld exceeds the 32-bit address of a key", (long long)n);
+  if (int rc = flat_check("tpq_flat_search", d, nq, n, ld)) return rc;
   TPQ_REQUIRE(values && ids && (address2id || n == 0), "tpq_flat_search: null output or address2id");
   if (nq == 0) return TPQ_OK;
-  TPQ_REQUIRE(x_dn, "tpq_flat_search: null query pointer");
-  TPQ_REQUIRE(n == 0 || (base && (norms || metric == TPQ_METRIC_INNER)), "tpq_flat_search: null base or norms");
-  const FlatPlan P = plan_flat(d, nq, n, k);
-  if (!ws || ws_bytes < P.total) {
-    set_error("tpq_flat_search: workspace too small (%zu < %zu)", ws_bytes, P.total);
-    return TPQ_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  uint64_t* keys = reinterpret_cast<uint64_t*>(w + P.keys);
-  float* xn = reinterpret_cast<float*>(w + P.xn);
-  const float* xq = x_dn;
-  if (metric == TPQ_METRIC_EUCLIDEAN) {
-    if (int rc = col_sqnorms(x_dn, d, nq, nq, xn, st)) return rc;
-  } else if (metric == TPQ_METRIC_COSINE) {
-    float* xs = reinterpret_cast<float*>(w + P.xq);
-    if (int rc = normalize_columns(x_dn, d, nq, kFlatEps, xs, st)) return rc;
-    xq = xs;
-  }
-  int rc;
-  switch (P.qt) {
-    case 16: rc = launch_flat<16>(metric, P, xq, d, nq, base, ld, n, norms, xn, k, keys, st); break;
-    case 32: rc = launch_flat<32>(metric, P, xq, d, nq, base, ld, n, norms, xn, k, keys, st); break;
-    default: rc = launch_flat<64>(metric, P, xq, d, nq, base, ld, n, norms, xn, k, keys, st); break;
-  }
-  if (rc) return rc;
+  FlatPlan P;
+  const float* xq;
+  if (int rc = flat_prepare("tpq_flat_search", x_dn, d, nq, base, n, norms, metric, k, ws, ws_bytes, st, P, xq))
+    return rc;
+  uint64_t* keys = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ws) + P.keys);
+  const float* xn = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + P.xn);
+  if (int rc = fused_launch<true>("flat_search_kernel", P.qt, metric, dim3(P.qtiles, P.S), P.smem, st,
+                                  [](auto q, auto m) { return flat_search_kernel<decltype(q)::value, decltype(m)::value>; },
+                                  xq, d, nq, base, ld, n, norms, xn, k, P.kp, P.slice_cols, keys))
+    return rc;
   // n == 0: every key is empty and the id table (capacity 0) is never read, so any non-null pointer will do
   return tpq_merge_topk(keys, nq, P.S, k, n ? address2id : reinterpret_cast<const int64_t*>(keys), n, values, ids,
                         address, stream);
@@ -298,7 +249,7 @@ extern "C" int tpq_flat_search(const float* x_dn, int d, int nq, const float* ba
 
 extern "C" size_t tpq_flat_range_workspace_bytes(int d, int nq, int64_t n) {
   if (d <= 0 || nq <= 0 || n < 0) return 0;
-  return plan_flat_range(d, nq, n).total;
+  return plan_flat(d, nq, n, 0).total;
 }
 
 extern "C" int tpq_flat_range_search(const float* x_dn, int d, int nq, const float* base, int64_t ld, int64_t n,
@@ -310,39 +261,21 @@ extern "C" int tpq_flat_range_search(const float* x_dn, int d, int nq, const flo
     return TPQ_ERR_UNSUPPORTED;
   }
   TPQ_REQUIRE(threshold == threshold, "tpq_flat_range_search: the threshold is NaN");
-  TPQ_REQUIRE(d > 0 && nq >= 0 && n >= 0 && ld >= n && cap >= 0,
-              "tpq_flat_range_search: bad sizes d=%d nq=%d n=%lld ld=%lld cap=%lld", d, nq, (long long)n, (long long)ld,
-              (long long)cap);
-  TPQ_REQUIRE(n < (int64_t(1) << 32), "tpq_flat_range_search: n=%lld exceeds the 32-bit address of a key", (long long)n);
+  TPQ_REQUIRE(cap >= 0, "tpq_flat_range_search: bad sizes d=%d nq=%d n=%lld ld=%lld cap=%lld", d, nq, (long long)n,
+              (long long)ld, (long long)cap);
+  if (int rc = flat_check("tpq_flat_range_search", d, nq, n, ld)) return rc;
   TPQ_REQUIRE(total && (cap == 0 || (match_keys && match_query)), "tpq_flat_range_search: null total or match buffer");
   if (nq == 0) return TPQ_OK;
-  TPQ_REQUIRE(x_dn, "tpq_flat_range_search: null query pointer");
-  TPQ_REQUIRE(n == 0 || (base && (norms || metric == TPQ_METRIC_INNER)), "tpq_flat_range_search: null base or norms");
-  const FlatRangePlan P = plan_flat_range(d, nq, n);
-  if (!ws || ws_bytes < P.total) {
-    set_error("tpq_flat_range_search: workspace too small (%zu < %zu)", ws_bytes, P.total);
-    return TPQ_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
+  FlatPlan P;
+  const float* xq;
+  if (int rc = flat_prepare("tpq_flat_range_search", x_dn, d, nq, base, n, norms, metric, 0, ws, ws_bytes, st, P, xq))
+    return rc;
   TPQ_CUDA(cudaMemsetAsync(total, 0, sizeof(uint64_t), st));
   if (n == 0) return TPQ_OK;
-  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  float* xn = reinterpret_cast<float*>(w + P.xn);
-  const float* xq = x_dn;
-  if (metric == TPQ_METRIC_EUCLIDEAN) {
-    if (int rc = col_sqnorms(x_dn, d, nq, nq, xn, st)) return rc;
-  } else if (metric == TPQ_METRIC_COSINE) {
-    float* xs = reinterpret_cast<float*>(w + P.xq);
-    if (int rc = normalize_columns(x_dn, d, nq, kFlatEps, xs, st)) return rc;
-    xq = xs;
-  }
-  unsigned long long* t = reinterpret_cast<unsigned long long*>(total);
-  switch (P.qt) {
-    case 16: return launch_flat_range<16>(metric, P, xq, d, nq, base, ld, n, norms, xn, threshold, match_keys,
-                                          match_query, cap, t, st);
-    case 32: return launch_flat_range<32>(metric, P, xq, d, nq, base, ld, n, norms, xn, threshold, match_keys,
-                                          match_query, cap, t, st);
-    default: return launch_flat_range<64>(metric, P, xq, d, nq, base, ld, n, norms, xn, threshold, match_keys,
-                                          match_query, cap, t, st);
-  }
+  const float* xn = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + P.xn);
+  return fused_launch<true>("flat_range_kernel", P.qt, metric, dim3(P.qtiles, P.S), P.smem, st,
+                            [](auto q, auto m) { return flat_range_kernel<decltype(q)::value, decltype(m)::value>; },
+                            xq, d, nq, base, ld, n, norms, xn, threshold, P.slice_cols, match_keys, match_query, cap,
+                            reinterpret_cast<unsigned long long*>(total));
 }

@@ -22,9 +22,8 @@
 // IVFSQIndex.search (tpq_ivfsq_search) is the same search over an SQCodec-coded store (word planes of 8-bit codes or
 // fp16): its scan instances read the codes through gemm_tile.cuh's BLoadSQ8 / BLoadSQ16, which decode them as the tile
 // stages them, so its scores are this search's over the decoded store, bit for bit.
-#include "gemm_tile.cuh"
+#include "fused_scan.cuh"
 #include "scan_layout.cuh"
-#include "range.cuh"
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k, const int64_t* address2id,
                               int64_t capacity, float* values, int64_t* ids, int64_t* address, void* stream);
@@ -32,28 +31,24 @@ extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int 
 namespace tpq {
 
 constexpr float kIvfFlatEps = 1e-8f;            // flat.cu's kFlatEps: metric.cosine_similarity's `norm + 1e-8`
-constexpr int kIvfFlatWarps = 8;
 constexpr size_t kIvfFlatKeyBytes = size_t(256) << 20;   // the chunk's keys [n_probe * S, n, k] stay within 256 MB
 constexpr int kIvfFlatMaxChunk = 16384;         // and a chunk holds at most this many queries
+constexpr size_t kIvfRangeXgBytes = size_t(256) << 20;   // the range search's gathered pair queries stay within 256 MB
 constexpr int kIvfFlatBuckets = 128;            // classes of the largest-first item order (4 per octave)
 constexpr int kIvfFlatMaxSlices = 128;          // n_probe * S parts per query at most (n_probe permitting)
 
-// Shared memory of one CTA, as flat.cu's: GEMM stages | score tile [QT][128] f32 | lists [QT][kp] | staging [8][kTopkBuf].
-static size_t ivfflat_smem_bytes(int qt, int kp) {
-  const size_t stages = 2 * (size_t)GK * (qt + GB) * 4;
-  return stages + (size_t)qt * GB * 4 + (size_t)qt * kp * 8 + (size_t)kIvfFlatWarps * kTopkBuf * 8;
-}
-
 // The plan, read by the workspace size and the search.  Every size is known before the search, from (d, nq, n_cells,
-// n_probe, k) alone:
-//   chunk0: queries per chunk when S = 1, the most whose keys fit kIvfFlatKeyBytes, at most kIvfFlatMaxChunk;
+// n_probe, k) alone; k == 0 is the range search's, with no lists and no keys:
+//   chunk0: queries per chunk when S = 1: the most whose keys fit kIvfFlatKeyBytes (k == 0: whose n_probe pair columns
+//           of d floats fit kIvfRangeXgBytes), at most kIvfFlatMaxChunk;
 //   QT:     16, 32 or 64: the smallest that holds a cell's expected pairs (chunk0 * n_probe / n_cells), halved while the
 //           shared memory exceeds 227 KB (k = 1024 gives 16, as in flat.cu);
 //   S:      column slices per (cell, query tile), enough for two CTAs per SM when the pairs make fewer tiles, with
 //           n_probe * S <= max(n_probe, 128) parts per query;
-//   chunk:  queries per chunk with S slices.
+//   chunk:  queries per chunk with S slices (k == 0: chunk0).
 // Per chunk of n queries: pairs = n * n_probe slots; the padded pair columns pad_cap = pairs + min(n_cells, pairs) *
 // (QT - 1) bound sum over cells of round_up(pairs of the cell, QT), and items = S * pad_cap / QT bounds the work items.
+// Past one chunk the workspace stops growing with nq.
 struct IvfFlatPlan {
   int qt, kp, S, chunk;
   int64_t pairs, pad_cap, items;
@@ -63,25 +58,25 @@ struct IvfFlatPlan {
 
 static IvfFlatPlan plan_ivfflat(int d, int nq, int n_cells, int n_probe, int k) {
   IvfFlatPlan P{};
-  P.kp = list_capacity(k);
-  const size_t per_query = (size_t)n_probe * k * 8;
-  auto chunk_of = [&](int S) {
-    size_t c = kIvfFlatKeyBytes / (per_query * S);
+  P.kp = k ? list_capacity(k) : 0;
+  auto chunk_of = [&](size_t budget, size_t per_query) {
+    size_t c = budget / per_query;
     c = c < (size_t)kIvfFlatMaxChunk ? c : (size_t)kIvfFlatMaxChunk;
     return (int)(c < 1 ? 1 : (c > (size_t)nq ? (size_t)nq : c));
   };
-  const int chunk0 = chunk_of(1);
+  const size_t keys_per_query = (size_t)n_probe * k * 8;
+  const int chunk0 = k ? chunk_of(kIvfFlatKeyBytes, keys_per_query) : chunk_of(kIvfRangeXgBytes, (size_t)n_probe * d * 4);
   const int64_t per_cell = ((int64_t)chunk0 * n_probe + n_cells - 1) / n_cells;
   P.qt = 16;
   while (P.qt < 64 && P.qt < per_cell) P.qt *= 2;
-  while (P.qt > 16 && ivfflat_smem_bytes(P.qt, P.kp) > kSmemLimit) P.qt /= 2;
-  P.smem = ivfflat_smem_bytes(P.qt, P.kp);
+  while (P.qt > 16 && fused_smem_bytes(P.qt, P.kp) > kSmemLimit) P.qt /= 2;
+  P.smem = fused_smem_bytes(P.qt, P.kp);
   const int64_t tiles = ((int64_t)chunk0 * n_probe + P.qt - 1) / P.qt;
   const int64_t want = 2 * (int64_t)device_sm_count();
   const int smax = n_probe >= kIvfFlatMaxSlices ? 1 : kIvfFlatMaxSlices / n_probe;
   int64_t S = tiles >= want ? 1 : (want + tiles - 1) / tiles;
   P.S = (int)(S > smax ? smax : S);
-  P.chunk = chunk_of(P.S);
+  P.chunk = k ? chunk_of(kIvfFlatKeyBytes, keys_per_query * P.S) : chunk0;
   P.pairs = (int64_t)P.chunk * n_probe;
   P.pad_cap = P.pairs + (P.pairs < n_cells ? P.pairs : n_cells) * (P.qt - 1);
   P.items = P.S * (P.pad_cap / P.qt);
@@ -256,7 +251,7 @@ ivfflat_scan_kernel(const float* __restrict__ xg, int d, int pad_cap, const int*
     bool live[4];
     #pragma unroll
     for (int u = 0; u < 4; ++u) live[u] = u * 32 + lane < cols && is_empty[c0 + u * 32 + lane] == 0;
-    for (int r = warp; r < rows; r += kIvfFlatWarps) {
+    for (int r = warp; r < rows; r += kFusedWarps) {
       WarpTopK tk{lists + (size_t)r * kp, wbuf, kp, k, 0};
       uint64_t thr = tk.kth();
       #pragma unroll
@@ -268,63 +263,11 @@ ivfflat_scan_kernel(const float* __restrict__ xg, int d, int pad_cap, const int*
     }
   }
   __syncthreads();                                     // the lists were last written by their own warps
-  for (int r = warp; r < rows; r += kIvfFlatWarps) {
+  for (int r = warp; r < rows; r += kFusedWarps) {
     const int p = p0 + r;
     uint64_t* dst = keys_out + (((size_t)pair_j[p] * S + sl) * n + pair_q[p]) * k;
     for (int i = lane; i < k; i += 32) dst[i] = lists[(size_t)r * kp + i];
   }
-}
-
-// ----------------------------------------------------------------------------- range search
-// tpq_ivfflat_range_search / tpq_ivfsq_range_search run steps 1-4 of every chunk as the search does, then
-// ivfflat_range_kernel, which keeps no lists: the scores above the threshold go to the match buffer of range.cuh.
-constexpr size_t kIvfRangeXgBytes = size_t(256) << 20;   // the chunk's gathered pair queries stay within 256 MB
-
-// Shared memory of one range CTA: GEMM stages | match buffer.  QT = 64: 24 + 81 = 105 KB, two CTAs per SM.
-static size_t ivfflat_range_smem_bytes(int qt) { return 2 * (size_t)GK * (qt + GB) * 4 + sizeof(RangeBuf); }
-
-// The range search's plan, read by its workspace size and the launches; the search's layout without keys:
-//   chunk: queries per chunk, the most whose n_probe pair columns of d floats fit kIvfRangeXgBytes, at most
-//          kIvfFlatMaxChunk -- the workspace stops growing with nq past one chunk;
-//   QT, S: as plan_ivfflat's for this chunk (no lists, so QT never halves).
-static IvfFlatPlan plan_ivfflat_range(int d, int nq, int n_cells, int n_probe) {
-  IvfFlatPlan P{};
-  size_t c = kIvfRangeXgBytes / ((size_t)n_probe * d * 4);
-  c = c < (size_t)kIvfFlatMaxChunk ? c : (size_t)kIvfFlatMaxChunk;
-  P.chunk = (int)(c < 1 ? 1 : (c > (size_t)nq ? (size_t)nq : c));
-  const int64_t per_cell = ((int64_t)P.chunk * n_probe + n_cells - 1) / n_cells;
-  P.qt = 16;
-  while (P.qt < 64 && P.qt < per_cell) P.qt *= 2;
-  P.smem = ivfflat_range_smem_bytes(P.qt);
-  const int64_t tiles = ((int64_t)P.chunk * n_probe + P.qt - 1) / P.qt;
-  const int64_t want = 2 * (int64_t)device_sm_count();
-  const int smax = n_probe >= kIvfFlatMaxSlices ? 1 : kIvfFlatMaxSlices / n_probe;
-  const int64_t S = tiles >= want ? 1 : (want + tiles - 1) / tiles;
-  P.S = (int)(S > smax ? smax : S);
-  P.pairs = (int64_t)P.chunk * n_probe;
-  P.pad_cap = P.pairs + (P.pairs < n_cells ? P.pairs : n_cells) * (P.qt - 1);
-  P.items = P.S * (P.pad_cap / P.qt);
-  const size_t n = (size_t)P.chunk;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += align_up(bytes, 256); return at; };
-  P.xc = take((size_t)d * n * 4);
-  P.xs = take((size_t)d * n * 4);
-  P.xp = take((size_t)d * n * 4);
-  P.xn = take(n * 4);
-  P.coarse_bytes = tpq_coarse_workspace_bytes(d, (int)n, n_cells);
-  P.coarse = take(P.coarse_bytes);
-  P.sims = take(n * n_probe * 4);
-  P.cells = take(n * n_probe * 8);
-  P.npl = take(n * 8);
-  P.cnt = take(((size_t)n_cells + 2) * 4);
-  P.off = take((size_t)n_cells * 4);
-  P.slot = take((size_t)P.pairs * 4);
-  P.pq = take((size_t)P.pad_cap * 4);
-  P.pj = take((size_t)P.pad_cap * 4);
-  P.itm = take((size_t)P.items * 16);
-  P.xg = take((size_t)d * P.pad_cap * 4);
-  P.total = o;
-  return P;
 }
 
 // One CTA per work item, as ivfflat_scan_kernel: the same GEMM, epilogue and is_empty mask, then every score > thr
@@ -425,9 +368,7 @@ static IvfChunk ivf_chunk_ws(const IvfFlatPlan& P, uint8_t* w) {
   return W;
 }
 
-// Steps 1-4 of the chunk [q0, q0 + n) of the batch, shared by the search and the range search: the chunk's queries, its
-// probe lists (the caller's, or the coarse probe's), |x|^2 (euclidean) or the normalised queries (cosine), the visited
-// pairs grouped by cell, the work items and the pairs' queries gathered into W.xg.
+// Steps 1-4 of ivf_chunks for the chunk [q0, q0 + n) of the batch.
 static int ivf_chunk_pairs(const IvfFlatPlan& P, uint8_t* w, const IvfChunk& W, const float* x_dn, int d, int nq, int q0,
                            int n, const float* vq_codebook, int n_cells, const int64_t* cells,
                            const int64_t* n_probe_list, int n_probe, int smart, float temperature, int metric,
@@ -471,6 +412,25 @@ static int ivf_chunk_pairs(const IvfFlatPlan& P, uint8_t* w, const IvfChunk& W, 
   return TPQ_OK;
 }
 
+// The batch in chunks of P.chunk queries, shared by the search and the range search.  For each chunk [q0, q0 + n):
+// steps 1-4 -- the chunk's queries, its probe lists (the caller's, or the coarse probe's), |x|^2 (euclidean) or the
+// normalised queries (cosine), the visited pairs grouped by cell, the work items and the pairs' queries gathered into
+// W.xg -- then scan(q0, n).
+template <class Scan>
+static int ivf_chunks(const IvfFlatPlan& P, uint8_t* w, const IvfChunk& W, const float* x_dn, int d, int nq,
+                      const float* vq_codebook, int n_cells, const int64_t* cells, const int64_t* n_probe_list,
+                      int n_probe, int smart, float temperature, int metric, const int64_t* cell_start,
+                      const int64_t* cell_size, cudaStream_t st, Scan scan) {
+  for (int q0 = 0; q0 < nq; q0 += P.chunk) {
+    const int n = nq - q0 < P.chunk ? nq - q0 : P.chunk;
+    if (int rc = ivf_chunk_pairs(P, w, W, x_dn, d, nq, q0, n, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart,
+                                 temperature, metric, cell_start, cell_size, st))
+      return rc;
+    if (int rc = scan(q0, n)) return rc;
+  }
+  return TPQ_OK;
+}
+
 // The checks of the search and the range search on the metric, the sizes and the probe lists.
 static int ivf_check(const char* name, int d, int nq, int n_cells, int n_probe, int64_t capacity, int metric,
                      const int64_t* cells, const int64_t* n_probe_list) {
@@ -488,22 +448,6 @@ static int ivf_check(const char* name, int d, int nq, int n_cells, int n_probe, 
     TPQ_REQUIRE(n_probe <= n_cells, "n_probe=%d must be in [1, n_cells=%d]", n_probe, n_cells);
     if (n_probe > 1024) { set_error("n_probe=%d > 1024 is not supported", n_probe); return TPQ_ERR_UNSUPPORTED; }
   }
-  return TPQ_OK;
-}
-
-template <int QT, class BL, class... Extra>
-static int launch_ivfflat_scan(int metric, const IvfFlatPlan& P, const float* xg, int d, const int* pair_q,
-                               const int* pair_j, const int4* items, const int* cnt, int n_cells, const int* off,
-                               const typename BL::T* storage, int64_t capacity, const uint8_t* is_empty,
-                               const int64_t* cell_start, const int64_t* cell_size, const float* norms, const float* xn,
-                               int n, int k, uint64_t* keys, cudaStream_t st, Extra... extra) {
-  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? ivfflat_scan_kernel<QT, TPQ_METRIC_EUCLIDEAN, BL, Extra...>
-                                             : ivfflat_scan_kernel<QT, TPQ_METRIC_COSINE, BL, Extra...>;
-  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
-  kern<<<(unsigned)P.items, 256, P.smem, st>>>(xg, d, (int)P.pad_cap, pair_q, pair_j, items, cnt, n_cells, off, storage,
-                                               capacity, is_empty, cell_start, cell_size, norms, xn, n, P.S, k, P.kp,
-                                               keys, extra...);
-  TPQ_LAUNCH_CHECK("ivfflat_scan_kernel");
   return TPQ_OK;
 }
 
@@ -532,35 +476,37 @@ static int ivf_search(const char* name, const float* x_dn, int d, int nq, const 
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
   uint64_t* keys = reinterpret_cast<uint64_t*>(w + P.keys);
   const IvfChunk W = ivf_chunk_ws(P, w);
-  float *xn = W.xn, *xg = W.xg;
-  int *cnt = W.cnt, *off = W.off, *pair_q = W.pair_q, *pair_j = W.pair_j;
-  int4* items = W.items;
   // capacity == 0: every key is empty and the id table is never read, so any non-null pointer will do
   const int64_t* a2i = capacity ? address2id : reinterpret_cast<const int64_t*>(keys);
-  for (int q0 = 0; q0 < nq; q0 += P.chunk) {
-    const int n = nq - q0 < P.chunk ? nq - q0 : P.chunk;
+  return ivf_chunks(P, w, W, x_dn, d, nq, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart, temperature, metric,
+                    cell_start, cell_size, st, [&](int q0, int n) {
     TPQ_CUDA(cudaMemsetAsync(keys, 0, (size_t)n_probe * P.S * n * k * 8, st));
-    if (int rc = ivf_chunk_pairs(P, w, W, x_dn, d, nq, q0, n, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart,
-                                 temperature, metric, cell_start, cell_size, st))
+    if (int rc = fused_launch<false>(
+            "ivfflat_scan_kernel", P.qt, metric, dim3((unsigned)P.items), P.smem, st,
+            [](auto q, auto m) { return ivfflat_scan_kernel<decltype(q)::value, decltype(m)::value, BL, Extra...>; },
+            W.xg, d, (int)P.pad_cap, W.pair_q, W.pair_j, W.items, W.cnt, n_cells, W.off, storage, capacity, is_empty,
+            cell_start, cell_size, norms, W.xn, n, P.S, k, P.kp, keys, extra...))
       return rc;
-    int rc;
-    switch (P.qt) {
-      case 16: rc = launch_ivfflat_scan<16, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
-                                                capacity, is_empty, cell_start, cell_size, norms, xn, n, k, keys, st,
-                                                extra...); break;
-      case 32: rc = launch_ivfflat_scan<32, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
-                                                capacity, is_empty, cell_start, cell_size, norms, xn, n, k, keys, st,
-                                                extra...); break;
-      default: rc = launch_ivfflat_scan<64, BL>(metric, P, xg, d, pair_q, pair_j, items, cnt, n_cells, off, storage,
-                                                capacity, is_empty, cell_start, cell_size, norms, xn, n, k, keys, st,
-                                                extra...); break;
-    }
-    if (rc) return rc;
-    if (int rc2 = tpq_merge_topk(keys, n, n_probe * P.S, k, a2i, capacity, values + (size_t)q0 * k,
-                                 ids + (size_t)q0 * k, address ? address + (size_t)q0 * k : nullptr, stream))
-      return rc2;
+    return tpq_merge_topk(keys, n, n_probe * P.S, k, a2i, capacity, values + (size_t)q0 * k, ids + (size_t)q0 * k,
+                          address ? address + (size_t)q0 * k : nullptr, stream);
+  });
+}
+
+// The checks of tpq_ivfsq_search and tpq_ivfsq_range_search on the code width, d and the 8-bit codec's lower and range,
+// then body(BLoadSQ16{}) or body(BLoadSQ8{}, lower, range): the loader and its own pointers.
+template <class Body>
+static int ivf_sq(const char* name, int bits, int d, const float* lower, const float* range, Body body) {
+  if (bits != 8 && bits != 16) {
+    set_error("%s: bits=%d is not supported (8 and 16 only)", name, bits);
+    return TPQ_ERR_UNSUPPORTED;
   }
-  return TPQ_OK;
+  TPQ_REQUIRE(d > 0 && d % (bits == 8 ? 4 : 2) == 0, "%s: d=%d must be a positive multiple of %d for %d bits", name, d,
+              bits == 8 ? 4 : 2, bits);
+  if (bits == 16) return body(BLoadSQ16{});
+  TPQ_REQUIRE(lower && range, "%s: null lower or range (8 bits)", name);
+  TPQ_REQUIRE((reinterpret_cast<uintptr_t>(lower) | reinterpret_cast<uintptr_t>(range)) % 16 == 0,
+              "%s: lower and range must be 16-byte aligned", name);
+  return body(BLoadSQ8{}, lower, range);
 }
 
 extern "C" int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
@@ -581,45 +527,18 @@ extern "C" int tpq_ivfsq_search(const float* x_dn, int d, int nq, const float* v
                                 const int64_t* n_probe_list, int n_probe, int smart, float temperature, int k,
                                 const int64_t* address2id, float* values, int64_t* ids, int64_t* address, void* ws,
                                 size_t ws_bytes, void* stream) {
-  if (bits != 8 && bits != 16) {
-    set_error("tpq_ivfsq_search: bits=%d is not supported (8 and 16 only)", bits);
-    return TPQ_ERR_UNSUPPORTED;
-  }
-  TPQ_REQUIRE(d > 0 && d % (bits == 8 ? 4 : 2) == 0, "tpq_ivfsq_search: d=%d must be a positive multiple of %d for %d bits",
-              d, bits == 8 ? 4 : 2, bits);
   const uint32_t* words = reinterpret_cast<const uint32_t*>(storage);
-  if (bits == 16)
-    return ivf_search<BLoadSQ16>("tpq_ivfsq_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
-                                 cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
-                                 temperature, k, address2id, values, ids, address, ws, ws_bytes, stream);
-  TPQ_REQUIRE(lower && range, "tpq_ivfsq_search: null lower or range (8 bits)");
-  TPQ_REQUIRE((reinterpret_cast<uintptr_t>(lower) | reinterpret_cast<uintptr_t>(range)) % 16 == 0,
-              "tpq_ivfsq_search: lower and range must be 16-byte aligned");
-  return ivf_search<BLoadSQ8>("tpq_ivfsq_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
-                              cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart, temperature,
-                              k, address2id, values, ids, address, ws, ws_bytes, stream, lower, range);
+  return ivf_sq("tpq_ivfsq_search", bits, d, lower, range, [&](auto bl, auto... extra) {
+    return ivf_search<decltype(bl)>("tpq_ivfsq_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
+                                    cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
+                                    temperature, k, address2id, values, ids, address, ws, ws_bytes, stream, extra...);
+  });
 }
 
 // ----------------------------------------------------------------------------- range search
 extern "C" size_t tpq_ivfflat_range_workspace_bytes(int d, int nq, int n_cells, int n_probe) {
   if (d <= 0 || nq <= 0 || n_cells <= 0 || n_probe <= 0) return 0;
-  return plan_ivfflat_range(d, nq, n_cells, n_probe).total;
-}
-
-template <int QT, class BL, class... Extra>
-static int launch_ivfflat_range(int metric, const IvfFlatPlan& P, const IvfChunk& W, int d, int n_cells,
-                                const typename BL::T* storage, int64_t capacity, const uint8_t* is_empty,
-                                const int64_t* cell_start, const int64_t* cell_size, const float* norms, float thr,
-                                int q_base, uint64_t* keys, int32_t* query, int64_t cap, unsigned long long* total,
-                                cudaStream_t st, Extra... extra) {
-  auto kern = metric == TPQ_METRIC_EUCLIDEAN ? ivfflat_range_kernel<QT, TPQ_METRIC_EUCLIDEAN, BL, Extra...>
-                                             : ivfflat_range_kernel<QT, TPQ_METRIC_COSINE, BL, Extra...>;
-  TPQ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem));
-  kern<<<(unsigned)P.items, 256, P.smem, st>>>(W.xg, d, (int)P.pad_cap, W.pair_q, W.items, W.cnt, n_cells, W.off,
-                                               storage, capacity, is_empty, cell_start, cell_size, norms, W.xn, P.S,
-                                               thr, q_base, keys, query, cap, total, extra...);
-  TPQ_LAUNCH_CHECK("ivfflat_range_kernel");
-  return TPQ_OK;
+  return plan_ivfflat(d, nq, n_cells, n_probe, 0).total;
 }
 
 // The body of tpq_ivfflat_range_search and tpq_ivfsq_range_search, as ivf_search is of the searches.
@@ -637,7 +556,7 @@ static int ivf_range(const char* name, const float* x_dn, int d, int nq, const f
   if (nq == 0) return TPQ_OK;
   TPQ_REQUIRE(x_dn && cell_start && cell_size && (cells || vq_codebook), "%s: null query or cell table", name);
   TPQ_REQUIRE(capacity == 0 || (storage && is_empty && norms), "%s: null store", name);
-  const IvfFlatPlan P = plan_ivfflat_range(d, nq, n_cells, n_probe);
+  const IvfFlatPlan P = plan_ivfflat(d, nq, n_cells, n_probe, 0);
   if (!ws || ws_bytes < P.total) {
     set_error("%s: workspace too small (%zu < %zu)", name, ws_bytes, P.total);
     return TPQ_ERR_WORKSPACE;
@@ -647,27 +566,15 @@ static int ivf_range(const char* name, const float* x_dn, int d, int nq, const f
   if (capacity == 0) return TPQ_OK;                    // nothing to score
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
   const IvfChunk W = ivf_chunk_ws(P, w);
-  unsigned long long* t = reinterpret_cast<unsigned long long*>(total);
-  for (int q0 = 0; q0 < nq; q0 += P.chunk) {
-    const int n = nq - q0 < P.chunk ? nq - q0 : P.chunk;
-    if (int rc = ivf_chunk_pairs(P, w, W, x_dn, d, nq, q0, n, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart,
-                                 temperature, metric, cell_start, cell_size, st))
-      return rc;
-    int rc;
-    switch (P.qt) {
-      case 16: rc = launch_ivfflat_range<16, BL>(metric, P, W, d, n_cells, storage, capacity, is_empty, cell_start,
-                                                 cell_size, norms, threshold, q0, match_keys, match_query, cap, t, st,
-                                                 extra...); break;
-      case 32: rc = launch_ivfflat_range<32, BL>(metric, P, W, d, n_cells, storage, capacity, is_empty, cell_start,
-                                                 cell_size, norms, threshold, q0, match_keys, match_query, cap, t, st,
-                                                 extra...); break;
-      default: rc = launch_ivfflat_range<64, BL>(metric, P, W, d, n_cells, storage, capacity, is_empty, cell_start,
-                                                 cell_size, norms, threshold, q0, match_keys, match_query, cap, t, st,
-                                                 extra...); break;
-    }
-    if (rc) return rc;
-  }
-  return TPQ_OK;
+  return ivf_chunks(P, w, W, x_dn, d, nq, vq_codebook, n_cells, cells, n_probe_list, n_probe, smart, temperature, metric,
+                    cell_start, cell_size, st, [&](int q0, int) {
+    return fused_launch<false>(
+        "ivfflat_range_kernel", P.qt, metric, dim3((unsigned)P.items), P.smem, st,
+        [](auto q, auto m) { return ivfflat_range_kernel<decltype(q)::value, decltype(m)::value, BL, Extra...>; },
+        W.xg, d, (int)P.pad_cap, W.pair_q, W.items, W.cnt, n_cells, W.off, storage, capacity, is_empty, cell_start,
+        cell_size, norms, W.xn, P.S, threshold, q0, match_keys, match_query, cap,
+        reinterpret_cast<unsigned long long*>(total), extra...);
+  });
 }
 
 extern "C" int tpq_ivfflat_range_search(const float* x_dn, int d, int nq, const float* vq_codebook, int n_cells,
@@ -689,21 +596,11 @@ extern "C" int tpq_ivfsq_range_search(const float* x_dn, int d, int nq, const fl
                                       const int64_t* n_probe_list, int n_probe, int smart, float temperature,
                                       float threshold, uint64_t* match_keys, int32_t* match_query, int64_t cap,
                                       uint64_t* total, void* ws, size_t ws_bytes, void* stream) {
-  if (bits != 8 && bits != 16) {
-    set_error("tpq_ivfsq_range_search: bits=%d is not supported (8 and 16 only)", bits);
-    return TPQ_ERR_UNSUPPORTED;
-  }
-  TPQ_REQUIRE(d > 0 && d % (bits == 8 ? 4 : 2) == 0,
-              "tpq_ivfsq_range_search: d=%d must be a positive multiple of %d for %d bits", d, bits == 8 ? 4 : 2, bits);
   const uint32_t* words = reinterpret_cast<const uint32_t*>(storage);
-  if (bits == 16)
-    return ivf_range<BLoadSQ16>("tpq_ivfsq_range_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity,
-                                is_empty, cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
-                                temperature, threshold, match_keys, match_query, cap, total, ws, ws_bytes, stream);
-  TPQ_REQUIRE(lower && range, "tpq_ivfsq_range_search: null lower or range (8 bits)");
-  TPQ_REQUIRE((reinterpret_cast<uintptr_t>(lower) | reinterpret_cast<uintptr_t>(range)) % 16 == 0,
-              "tpq_ivfsq_range_search: lower and range must be 16-byte aligned");
-  return ivf_range<BLoadSQ8>("tpq_ivfsq_range_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity, is_empty,
-                             cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart, temperature,
-                             threshold, match_keys, match_query, cap, total, ws, ws_bytes, stream, lower, range);
+  return ivf_sq("tpq_ivfsq_range_search", bits, d, lower, range, [&](auto bl, auto... extra) {
+    return ivf_range<decltype(bl)>("tpq_ivfsq_range_search", x_dn, d, nq, vq_codebook, n_cells, words, capacity,
+                                   is_empty, cell_start, cell_size, norms, metric, cells, n_probe_list, n_probe, smart,
+                                   temperature, threshold, match_keys, match_query, cap, total, ws, ws_bytes, stream,
+                                   extra...);
+  });
 }

@@ -169,14 +169,17 @@ class FlatIndex(IdContainer):
             self._norms = (key, table)
         return self._norms[1]
 
-    def search(self, x, k=1, return_address=False):
-        """FlatIndex.search (FlatIndex.py:46-101): x [d_vector, n_query] fp32 on the index device
-        -> (topk_values [n_query, k] fp32 descending, topk_ids [n_query, k] int64[, topk_address])."""
+    def _check_query(self, x):
         assert x.dim() == 2 and x.shape[0] == self.d_vector
         assert x.dtype == torch.float32 and x.device == self._storage.device
         assert x.device.type == "cuda", "torchpq_b200 has no CPU path: the index must live on a CUDA device"
+        return x.contiguous()
+
+    def search(self, x, k=1, return_address=False):
+        """FlatIndex.search (FlatIndex.py:46-101): x [d_vector, n_query] fp32 on the index device
+        -> (topk_values [n_query, k] fp32 descending, topk_ids [n_query, k] int64[, topk_address])."""
+        x = self._check_query(x)
         assert k >= 1
-        x = x.contiguous()
         dev, nq = x.device, x.shape[1]
         values = torch.empty(nq, k, dtype=torch.float32, device=dev)
         ids = torch.empty(nq, k, dtype=torch.long, device=dev)
@@ -203,11 +206,8 @@ class FlatIndex(IdContainer):
         ``distance < r^2`` is ``threshold = -r^2``.  More than `max_results` matches raise ValueError (naming the
         total) and return nothing.  Unlike search, this synchronises the stream once, to read the number of matches.
         """
-        assert x.dim() == 2 and x.shape[0] == self.d_vector
-        assert x.dtype == torch.float32 and x.device == self._storage.device
-        assert x.device.type == "cuda", "torchpq_b200 has no CPU path: the index must live on a CUDA device"
+        x = self._check_query(x)
         t = _range.threshold_f32(threshold)
-        x = x.contiguous()
         dev, nq, n = x.device, x.shape[1], self._n_items
         if nq == 0:
             return _range.empty(0, dev, return_address)

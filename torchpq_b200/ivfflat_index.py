@@ -22,6 +22,8 @@ from .modules import Codec, IdContainer, _fingerprint
 
 
 class IVFFlatIndex(IdContainer):
+    _SEARCH, _RANGE = "tpq_ivfflat_search", "tpq_ivfflat_range_search"       # the library's entry points
+
     def __init__(self, d_vector, n_cells=128, initial_size=None, expand_step_size=128, expand_mode="double",
                  distance="euclidean", device="cuda:0", verbose=0):
         super().__init__()
@@ -65,6 +67,10 @@ class IVFFlatIndex(IdContainer):
     def _empty_store(self, cap, dev):
         """A zero store of `cap` slots: fp32 [d, cap, 1]."""
         return torch.zeros(self.d_vector, cap, 1, dtype=torch.float32, device=dev)
+
+    def _store_args(self):
+        """The store's arguments of the search entry points, between n_cells and capacity."""
+        return (ptr(self._storage),)
 
     def load_state_dict(self, state_dict, strict=True):
         """As IVFPQIndex.load_state_dict: the buffers, then ``_max_id`` re-derived and holes assumed."""
@@ -150,18 +156,14 @@ class IVFFlatIndex(IdContainer):
         ws_bytes = lib.tpq_ivfflat_workspace_bytes(self.d_vector, nq, self.n_cells, n_probe, k)
         ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
         vq = self.vq_codec.kmeans.centroids if cells is None else None
-        entry, store = self._search_entry()
-        check(entry(ptr(x), self.d_vector, nq, ptr(vq), self.n_cells, *store, self.capacity,
+        entry = getattr(lib, self._SEARCH)
+        check(entry(ptr(x), self.d_vector, nq, ptr(vq), self.n_cells, *self._store_args(), self.capacity,
                     ptr(self._is_empty), ptr(self._cell_start), ptr(self._cell_size), ptr(norms),
                     _lib.METRIC[self.distance], ptr(cells), ptr(n_probe_list), n_probe,
                     int(bool(self.use_smart_probing)), float(self.smart_probing_temperature), k,
                     ptr(self._address2id), ptr(values), ptr(ids), ptr(address), ptr(ws), ws_bytes,
                     _lib.current_stream(dev)))
         return out
-
-    def _search_entry(self):
-        """(the library's search entry point, its store arguments between n_cells and capacity)."""
-        return lib.tpq_ivfflat_search, (ptr(self._storage),)
 
     def search(self, x, k=1, return_address=False):
         """x [d_vector, n_query] fp32 on the index device -> (values [n_query, k] fp32 descending, ids [n_query, k]
@@ -191,7 +193,7 @@ class IVFFlatIndex(IdContainer):
         norms = self._norm_table()
         ws_bytes = lib.tpq_ivfflat_range_workspace_bytes(self.d_vector, nq, self.n_cells, n_probe)
         ws = torch.empty(max(1, ws_bytes), dtype=torch.uint8, device=dev)
-        entry, store = self._range_entry()
+        entry, store = getattr(lib, self._RANGE), self._store_args()
 
         def run(keys, query, cap, total):
             check(entry(ptr(x), self.d_vector, nq, ptr(self.vq_codec.kmeans.centroids), self.n_cells, *store,
@@ -200,10 +202,6 @@ class IVFFlatIndex(IdContainer):
                         float(self.smart_probing_temperature), t, ptr(keys), ptr(query), cap, ptr(total), ptr(ws),
                         ws_bytes, _lib.current_stream(dev)))
         return _range.collect(run, nq, max_results, self._address2id, return_address, dev)
-
-    def _range_entry(self):
-        """(the library's range search entry point, its store arguments between n_cells and capacity)."""
-        return lib.tpq_ivfflat_range_search, (ptr(self._storage),)
 
     def search_cells(self, x, cells, n_probe_list=None, k=1, return_address=False):
         """As IVFPQIndex.search_cells: cells [n_query, n_probe] int64 probe lists, n_probe_list [n_query] int64

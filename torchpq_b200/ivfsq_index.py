@@ -26,6 +26,8 @@ _NORM_CHUNK = 1 << 16            # slots decoded at a time by the norm table's b
 
 
 class IVFSQIndex(IVFFlatIndex):
+    _SEARCH, _RANGE = "tpq_ivfsq_search", "tpq_ivfsq_range_search"
+
     def __init__(self, d_vector, n_cells=128, bits=8, sq_mode="minmax", sq_alpha=1.0, initial_size=None,
                  expand_step_size=128, expand_mode="double", distance="euclidean", device="cuda:0", verbose=0):
         if bits not in (8, 16):
@@ -123,12 +125,7 @@ class IVFSQIndex(IVFFlatIndex):
             self._norms = (key, table)
         return self._norms[1]
 
-    def _search_entry(self):
+    def _store_args(self):
         lo, rg = self.sq_codec._bounds(self._storage.device)               # None for 16 bits
         self._sq_bounds = (lo, rg)                                       # kept alive past the launch
-        return lib.tpq_ivfsq_search, (ptr(self._storage), self.bits, ptr(lo), ptr(rg))
-
-    def _range_entry(self):
-        lo, rg = self.sq_codec._bounds(self._storage.device)
-        self._sq_bounds = (lo, rg)
-        return lib.tpq_ivfsq_range_search, (ptr(self._storage), self.bits, ptr(lo), ptr(rg))
+        return ptr(self._storage), self.bits, ptr(lo), ptr(rg)
