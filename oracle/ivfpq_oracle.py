@@ -98,12 +98,13 @@ def get_ioa(cells: np.ndarray) -> np.ndarray:
 
 def _expand(st: IndexState, cells: np.ndarray, expand_mode="double", expand_step_size=128):
     """CellContainer.expand (CellContainer.py:249-311): insert a block of fresh slots
-    right after each listed cell and shift every later cell."""
+    right after each listed cell and shift every later cell.  A cell of capacity 0 grows
+    by expand_step_size in "double" mode too (the reference doubles it to 0, forever)."""
     for c in cells:
         c = int(c)
         start, cap = int(st.cell_start[c]), int(st.cell_capacity[c])
         end = start + cap
-        n_new = cap if expand_mode == "double" else expand_step_size
+        n_new = (cap or expand_step_size) if expand_mode == "double" else expand_step_size
         st.storage = np.concatenate(
             [st.storage[:, :end], np.zeros((st.storage.shape[0], n_new, 4), np.uint8), st.storage[:, end:]], axis=1)
         st.address2id = np.concatenate([st.address2id[:end], -np.ones(n_new, np.int64), st.address2id[end:]])

@@ -3,6 +3,7 @@ cell-major or query-major) changes speed, not results, so a wrong choice would p
 choice for each kind of index by the kernels a single search launches, as torch.profiler records them."""
 import ctypes as C
 import re
+import time
 
 import pytest
 import torch
@@ -21,24 +22,39 @@ CELL = {"cell_lut_kernel<2>", "ivfpq_scan_kernel<64, 8, 2, 0, false>", "ivfpq_ce
         "merge_topk_kernel"}
 
 
-def launched(fn, windows=3):
+def launched(fn, windows=3, max_windows=12):
     """names (namespace and parameter list stripped) of the scan, LUT, cell and merge kernels that fn() launches.
-    Late in a long pytest process the profiler has dropped the first launch of a window, and now and then every launch
-    of one; so each window opens with a throwaway kernel, and the names seen in a few windows are pooled (fn() launches
-    the same kernels on every call)."""
+    The profiler keeps only the device events whose timestamps fall inside its window, and its device timestamps drift
+    from its host clock as a process ages: late in a long pytest process it drops the first launches of a window, then
+    every launch of it; and now and then a window loses its device events altogether.  So fn() runs between two marker
+    kernels, with a pause on either side of them that doubles whenever a marker goes missing; a window counts when it
+    recorded both markers (so nothing between them fell outside it), and the names seen in `windows` such windows are
+    pooled (fn() launches the same kernels on every call, and a dropped event can only hide a name, never add one)."""
     fn()                                                                  # layout, module loads
     torch.cuda.synchronize()
-    names = set()
-    for _ in range(windows):
+    names, complete, pad = set(), 0, 0.05
+    for _ in range(max_windows):
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            torch.ones(1, device="cuda").add_(1)
+            time.sleep(pad)
+            torch.cuda._sleep(1000)                                       # marker: spin_kernel
             torch.cuda.synchronize()
             fn()
             torch.cuda.synchronize()
+            torch.cuda._sleep(1000)
+            torch.cuda.synchronize()
+            time.sleep(pad)
+        markers = 0
         for e in prof.events():
+            markers += e.device_type == torch.autograd.DeviceType.CUDA and "spin_kernel" in e.name
             n = re.sub(r"^void ", "", e.name).replace("tpq::", "").split("(")[0]
             if any(s in n for s in ("scan", "lut", "cell_", "merge")):
                 names.add(n)
+        if markers == 2:
+            complete += 1
+            if complete == windows:
+                break
+        else:
+            pad = min(2 * pad, 3.2)
     return names
 
 

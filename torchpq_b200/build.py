@@ -138,17 +138,29 @@ def _expand(index, grow: torch.Tensor):
     shift = torch.cumsum(grow, 0) - grow                           # slots inserted before each cell
     old_cap = index.capacity
     new_cap = old_cap + int(grow.sum().item())
+    if new_cap == old_cap:                                         # container_add would repeat this round forever
+        raise RuntimeError("container expansion made no room: a short cell grew by 0 slots")
     storage = index._storage.new_zeros((index._storage.shape[0], new_cap, index._storage.shape[2]))   # u8 codes or f32
     a2i = torch.full((new_cap,), -1, dtype=torch.long, device=dev)
     emp = torch.ones(new_cap, dtype=torch.uint8, device=dev)
-    check(lib.tpq_expand_move(ptr(index._storage), ptr(index._address2id), ptr(index._is_empty), ptr(index._cell_start),
-                              ptr(shift), index.n_cells, index.code_size, old_cap, new_cap,
-                              ptr(storage), ptr(a2i), ptr(emp), _lib.current_stream(dev)))
+    if old_cap > 0:                                                # an empty store has no slot to move (and no pointers)
+        check(lib.tpq_expand_move(ptr(index._storage), ptr(index._address2id), ptr(index._is_empty), ptr(index._cell_start),
+                                  ptr(shift), index.n_cells, index.code_size, old_cap, new_cap,
+                                  ptr(storage), ptr(a2i), ptr(emp), _lib.current_stream(dev)))
     for name, val in (("_storage", storage), ("_address2id", a2i), ("_is_empty", emp)):
         delattr(index, name)
         index.register_buffer(name, val)
     index._cell_start += shift
     index._cell_capacity += grow
+
+
+def growth(capacity: torch.Tensor, short: torch.Tensor, expand_mode: str, expand_step_size: int) -> torch.Tensor:
+    """Slots one expansion round adds to each cell (CellContainer.expand, CellContainer.py:249-311): 0 where the cell
+    has room; for a short cell its capacity ("double") or expand_step_size ("step").  A cell of capacity 0 cannot
+    double -- the reference's loop never ends on one -- so in "double" mode it grows by expand_step_size instead."""
+    step = torch.full_like(capacity, expand_step_size)
+    grow = torch.where(capacity > 0, capacity, step) if expand_mode == "double" else step
+    return torch.where(short, grow, torch.zeros_like(capacity))
 
 
 def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, return_address=False):
@@ -183,8 +195,9 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
     while True:
         # free slots of a cell = capacity - LIVE items.  Without holes live == _cell_size and this is the reference's
         # `capacity - cell_size - (ioa + 1) < 0` test (CellContainer.py:338-341) taken per cell: the largest ioa of a cell
-        # is its count - 1.  With holes left by remove() the empty-slot prefix gives the live count.
-        if index._has_holes:
+        # is its count - 1.  With holes left by remove() the empty-slot prefix gives the live count.  A store of
+        # capacity 0 (initial_size=0, or such a checkpoint loaded) holds nothing: every _cell_size is 0.
+        if index._has_holes and index.capacity > 0:
             prefix = fn.empty_prefix(index._is_empty)
             p = prefix.to(torch.long) & 0xFFFFFFFF
             live = index._cell_capacity - (p[index._cell_start + index._cell_capacity] - p[index._cell_start])
@@ -193,9 +206,7 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
         short = counts > index._cell_capacity - live
         if not bool(short.any().item()):
             break
-        grow = torch.where(short, index._cell_capacity if index.expand_mode == "double"
-                           else torch.full_like(index._cell_capacity, index.expand_step_size), torch.zeros_like(counts))
-        _expand(index, grow)
+        _expand(index, growth(index._cell_capacity, short, index.expand_mode, index.expand_step_size))
         in_sync = False                                              # addresses moved: the scan layout is rebuilt lazily
     write = fn.get_write_address(cells, ioa, index._cell_start, index._cell_size, index._cell_capacity, prefix)
     ix = lay.cindex if in_sync else _lib.TpqIndex()
@@ -209,6 +220,7 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
                               ptr(index._storage), ptr(index._address2id), ptr(index._is_empty), ptr(index._cell_size),
                               ptr(lay.codes_scan) if in_sync else None, ptr(lay.block_valid) if in_sync else None,
                               _lib.current_stream(dev)))
+    index._ids_changed()                                             # the kernel wrote _address2id past its _version
     index._max_id = max(index._max_id, int(ids.max().item()))
     if in_sync:                                                      # the layout received the same items and stays valid
         rank, world = lay.shard                                      # (raw-pointer writes do not move the buffers' fingerprint);

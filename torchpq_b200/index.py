@@ -201,6 +201,8 @@ class IVFPQIndex(IdContainer):
         self.vq_codec.set_codebook(T(st.vq_codebook))
         self.pq_codec.set_codebook(T(st.pq_codebook))
         self._max_id = int(st.max_id)
+        self._has_holes = True                                          # as load_state_dict: the state may have holes
+        self._ids_changed()                                             # a new _address2id may reuse the old one's memory
         self.n_probe = st.n_probe
         self.use_smart_probing = st.use_smart_probing
         self.smart_probing_temperature = st.smart_probing_temperature

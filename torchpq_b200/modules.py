@@ -43,8 +43,14 @@ class IdContainer(StateModule):
     """The id bookkeeping of BaseContainer (container/BaseContainer.py:30-110) that IVFPQIndex and FlatIndex share: the
     ``_address2id`` / ``_id2address`` buffers, ``capacity``, ``max_id`` (tracked, and re-derived from ``_address2id``
     after a checkpoint load, where the reference restarts it at -1) and the two lookups.  The inverse map is rebuilt
-    lazily, whenever ``_address2id`` has changed since it was built.  Subclasses register both buffers and set
-    ``_max_id = -1`` and ``_id2address_fp = None``."""
+    lazily, whenever ``_address2id`` has changed since it was built: its fingerprint (pointer, ``_version``, shape) sees
+    every write through torch, and a writer that bypasses ``_version`` (a kernel writing through the raw pointer,
+    build.container_add) calls ``_ids_changed``.  Subclasses register both buffers and set ``_max_id = -1`` and
+    ``_id2address_fp = None``."""
+
+    def _ids_changed(self):
+        """``_address2id`` was written where its ``_version`` does not see it: drop the inverse map."""
+        self._id2address_fp = None
 
     @property
     def capacity(self):
@@ -57,7 +63,7 @@ class IdContainer(StateModule):
     def _refresh_max_id(self):
         a2i = self._address2id
         self._max_id = int(a2i.max().item()) if a2i is not None and a2i.numel() else -1
-        self._id2address_fp = None
+        self._ids_changed()
 
     def get_id_by_address(self, address):
         """BaseContainer.get_id_by_address (BaseContainer.py:58-65) -- plain tensor indexing, not on the hot path."""
@@ -82,7 +88,8 @@ class IdContainer(StateModule):
             delattr(self, "_id2address")
             self.register_buffer("_id2address", id2a)
             self._id2address_fp = _fingerprint(self._address2id)
-        mask = (0 <= ids) & (ids <= self._max_id)
+        # bounded by the map's own length too: a lookup can never index past it, even were the map stale
+        mask = (0 <= ids) & (ids <= self._max_id) & (ids < self._id2address.shape[0])
         address = torch.ones_like(ids) * -1
         address[mask] = self._id2address[ids[mask]]
         return address
