@@ -16,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import lib, check, ptr
-from .modules import StateModule
+from .modules import StateModule, on_device
 
 __all__ = ["SQCodec"]
 
@@ -83,6 +83,7 @@ class SQCodec(StateModule):
         assert lo.device == device and rg.device == device, "the codec's buffers live on another device"
         return _aligned(lo), _aligned(rg)
 
+    @on_device(lambda self, x: x.device)
     def encode(self, x):
         """x [d_vector, n] fp32 CUDA -> [d_vector, n] u8 (bits 8), fp16 (bits 16), or x itself (bits 32)."""
         assert self.is_trained, "codec is not trained"
@@ -98,6 +99,7 @@ class SQCodec(StateModule):
         check(lib.tpq_sq_encode(ptr(x), d, n, self.bits, ptr(lo), ptr(rg), ptr(out), _lib.current_stream(x.device)))
         return out
 
+    @on_device(lambda self, code: code.device)
     def decode(self, code):
         """code [d_vector, n] u8 (bits 8), fp16 (bits 16) or fp32 (bits 32, returned as is) -> [d_vector, n] fp32."""
         assert self.is_trained, "codec is not trained"

@@ -19,7 +19,7 @@ import torch
 
 from . import _lib, _range
 from ._lib import lib, check, ptr
-from .modules import IdContainer, _fingerprint
+from .modules import IdContainer, StreamCache, _fingerprint, on_index_device
 
 _DISTANCE = {"euclidean": "euclidean", "l2": "euclidean", "cosine": "cosine", "angular": "cosine",
              "inner": "inner", "dot": "inner"}                     # FlatIndex.py:31-40
@@ -105,6 +105,7 @@ class FlatIndex(IdContainer):
         self._storage[:, address[mask], 0] = data[:, mask]
         self._state_changed()
 
+    @on_index_device
     def add(self, x, ids=None, return_address=False):
         """FlatContainer.add (FlatContainer.py:118-158): x [d, n] goes to addresses [n_items, n_items + n); default ids
         continue after max_id."""
@@ -127,6 +128,7 @@ class FlatIndex(IdContainer):
         self._state_changed()
         return (ids, address) if return_address else ids
 
+    @on_index_device
     def remove(self, ids=None, address=None):
         """FlatContainer.remove (FlatContainer.py:160-190): the store stays a prefix -- the surviving items of the last
         n_removed slots move, in ascending order, into the removed slots below them.  Addresses outside the live
@@ -166,8 +168,8 @@ class FlatIndex(IdContainer):
             table = torch.empty(max(1, n), dtype=torch.float32, device=dev)
             check(lib.tpq_flat_norms(ptr(self._storage), self.capacity, self.d_vector, n, _lib.METRIC[self.distance],
                                      ptr(table), _lib.current_stream(dev)))
-            self._norms = (key, table)
-        return self._norms[1]
+            self._norms = (key, StreamCache(table, dev))
+        return self._norms[1].get()
 
     def _check_query(self, x):
         assert x.dim() == 2 and x.shape[0] == self.d_vector
@@ -175,6 +177,7 @@ class FlatIndex(IdContainer):
         assert x.device.type == "cuda", "torchpq_b200 has no CPU path: the index must live on a CUDA device"
         return x.contiguous()
 
+    @on_index_device
     def search(self, x, k=1, return_address=False):
         """FlatIndex.search (FlatIndex.py:46-101): x [d_vector, n_query] fp32 on the index device
         -> (topk_values [n_query, k] fp32 descending, topk_ids [n_query, k] int64[, topk_address])."""
@@ -195,6 +198,7 @@ class FlatIndex(IdContainer):
                                   ptr(address), ptr(ws), ws_bytes, _lib.current_stream(dev)))
         return out
 
+    @on_index_device
     def range_search(self, x, threshold, return_address=False, max_results=1 << 26):
         """Every live item scoring above `threshold`: x [d_vector, n_query] fp32 on the index device, threshold a float
         or a 0-d tensor (rounded once to fp32; NaN raises ValueError)

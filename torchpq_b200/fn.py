@@ -13,6 +13,7 @@ import torch
 
 from . import _lib
 from ._lib import lib, check, ptr
+from .modules import on_data_device, on_device
 
 
 def _cuda_f32(t, name):
@@ -21,6 +22,7 @@ def _cuda_f32(t, name):
     return t.contiguous()
 
 
+@on_data_device
 def normalize(x, dim=0):
     """util.normalize for a [d, n] matrix along dim 0: x / (||x|| + 1e-9)."""
     assert dim == 0 and x.dim() == 2
@@ -30,6 +32,7 @@ def normalize(x, dim=0):
     return out
 
 
+@on_data_device
 def coarse_probe(x, vq_codebook, n_probe, use_smart_probing=True, smart_probing_temperature=30.0):
     """x [d, nq], vq_codebook [d, n_cells] -> (topk_sims [nq, n_probe] desc, cells [nq, n_probe] i64,
     n_probe_list [nq] i64)."""
@@ -49,6 +52,7 @@ def coarse_probe(x, vq_codebook, n_probe, use_smart_probing=True, smart_probing_
     return sims, cells, npl
 
 
+@on_data_device
 def precompute_adc(query, pq_codebook, distance="euclidean"):
     """PQCodec.precompute_adc: query [d, nq], pq_codebook [M, dsub, 256] -> [M, nq, 256] fp32."""
     q, cb = _cuda_f32(query, "query"), _cuda_f32(pq_codebook, "pq_codebook")
@@ -68,6 +72,7 @@ class IVFPQTopk:
         assert contiguous_size == 4
         self.n_subvectors = n_subvectors
 
+    @on_device(lambda self, data, *a, **k: data.device)
     def topk(self, data, precomputed, cell_start, cell_size, is_empty, n_probe_list, k=256):
         assert 0 < k <= 1024                                             # fn/IVFPQTopk.py:64
         n_data = data.shape[1]
@@ -93,6 +98,7 @@ class IVFPQTopk:
         return values, address
 
 
+@on_data_device
 def max_sim(data, centroids, distance="euclidean", exact=True, exact_values=True):
     """MultiKMeans.get_labels / MaxSimCuda(dim=2): data [l, d, n], centroids [l, d, k] ->
     (maxsims [l, n] f32, labels [l, n] i64); distance "euclidean", "cosine" (inner product) or "manhattan".  exact=False lets the TF32 tensor-core kernel run where it applies;
@@ -108,6 +114,7 @@ def max_sim(data, centroids, distance="euclidean", exact=True, exact_values=True
     return sims, labels
 
 
+@on_data_device
 def kmeans_assign(data, centroids, distance="euclidean", exact_values=True):
     """The assignment step of KMeans / MultiKMeans: data [l, d, n], centroids [l, d, k] -> (maxsims [l, n] f32,
     labels [l, n] i64), on the TF32 tensor-core kernels wherever one takes the shape (tpq_kmeans_assign in
@@ -126,6 +133,7 @@ def kmeans_assign(data, centroids, distance="euclidean", exact_values=True):
     return sims, labels
 
 
+@on_data_device
 def compute_centroids(data, labels, k):
     """ComputeCentroidsCuda.__call__: data [l, d, n], labels [l, n] i64 -> centroids [l, d, k]."""
     a = _cuda_f32(data, "data")
@@ -140,6 +148,7 @@ def compute_centroids(data, labels, k):
     return cent
 
 
+@on_data_device
 def pq_decode(codebook, code):
     """PQDecodeCuda.__call__: codebook [M, dsub, 256], code [M, n] u8 -> [M*dsub, n] f32."""
     cb = _cuda_f32(codebook, "codebook")
@@ -152,6 +161,7 @@ def pq_decode(codebook, code):
     return out
 
 
+@on_data_device
 def merge_topk(keys, address2id):
     """keys [n_parts, nq, k] int64-viewed packed candidates (each part sorted) -> (values, ids, address)."""
     assert keys.dim() == 3 and keys.dtype == torch.int64 and keys.is_contiguous()
@@ -173,6 +183,7 @@ class Topk:
     (-inf, -1).  k > 1024 raises NotImplementedError (the reference falls back to torch.topk; this package has no
     torch fallback)."""
 
+    @on_device(lambda self, x, *a, **k: x.device)
     def __call__(self, x, k=1, dim=1):
         if dim == -1:
             dim = 1
@@ -192,13 +203,12 @@ class Topk:
         indices = torch.empty(m, k, dtype=torch.int64, device=dev)
         ws_bytes = lib.tpq_topk_workspace_bytes(m, n, k, dtype)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
-        with torch.cuda.device(dev):
-            check(lib.tpq_topk(ptr(x), m, n, dtype, k, ptr(values), ptr(indices), ptr(ws), ws_bytes,
-                               _lib.current_stream(dev)))
+        check(lib.tpq_topk(ptr(x), m, n, dtype, k, ptr(values), ptr(indices), ptr(ws), ws_bytes, _lib.current_stream(dev)))
         return values.to(x.dtype), indices
 
 
 # ------------------------------------------------------------------ build side (CellContainer.add, CellContainer.py:313-367)
+@on_data_device
 def get_ioa(cells, n_cells):
     """get_ioa (kernels/cuda/get_ioa.cu:8-47): cells [n] i64 -> (ioa [n] i64, counts [n_cells] i64)."""
     assert cells.dtype == torch.int64 and cells.dim() == 1 and cells.device.type == "cuda"
@@ -212,6 +222,7 @@ def get_ioa(cells, n_cells):
     return ioa, counts
 
 
+@on_data_device
 def empty_prefix(is_empty):
     """prefix[a] = number of empty slots in [0, a), a = 0..capacity  (int32-viewed uint32)."""
     assert is_empty.dtype == torch.uint8 and is_empty.device.type == "cuda"
@@ -224,6 +235,7 @@ def empty_prefix(is_empty):
     return prefix
 
 
+@on_data_device
 def get_write_address(cells, ioa, cell_start, cell_size, cell_capacity, prefix=None):
     """get_write_address (kernels/cuda/get_write_address_v2.cu:9-41): the ioa-th empty slot of each item's cell."""
     n, dev = cells.shape[0], cells.device

@@ -18,7 +18,7 @@ import torch
 
 from . import _lib, _range
 from ._lib import lib, check, ptr
-from .modules import Codec, IdContainer, _fingerprint
+from .modules import Codec, IdContainer, StreamCache, _fingerprint, on_index_device
 
 
 def _codebook_of(codec):
@@ -99,9 +99,7 @@ class ScanLayout:
         popc = torch.tensor([bin(i).count("1") for i in range(256)], dtype=torch.long, device=dev)
         self.set_live(int(popc[bits].sum().item()) if self.n_blocks else 0)
         self.fingerprint = _fingerprint(*self.keep)
-        self.stream_id = (stream.value or 0)                                  # searches on another stream wait on `ready`
-        self.ready = torch.cuda.Event()
-        self.ready.record(torch.cuda.current_stream(dev))
+        self.ready = StreamCache(None, dev)                              # a search on another stream waits for the kernels above
 
     def set_live(self, n_live: int) -> None:
         self.n_live = n_live
@@ -238,6 +236,7 @@ class IVFPQIndex(IdContainer):
         n = sum(t.numel() * t.element_size() for t in self.buffers() if t is not None)
         return n + (self._layout.resident_bytes() if self._layout is not None else 0)
 
+    @on_index_device
     def layout(self) -> ScanLayout:
         vq, pq = _codebook_of(self.vq_codec), _codebook_of(self.pq_codec)     # no host sync (is_trained.item()) per search
         fp = _fingerprint(self._storage, self._is_empty, self._cell_start, self._cell_size, self._address2id, vq, pq)
@@ -245,11 +244,8 @@ class IVFPQIndex(IdContainer):
             assert self._storage is not None, "shard-only index: its state cannot change (re-distribute the full index)"
             assert self.vq_codec.is_trained and self.pq_codec.is_trained, "codec is not trained"
             self._layout = ScanLayout(self, *self._shard)
-        lay = self._layout
-        cur = torch.cuda.current_stream(self._address2id.device)
-        if lay.ready is not None and cur.cuda_stream != lay.stream_id:
-            cur.wait_event(lay.ready)                                  # layout kernels ran on another stream
-        return lay
+        self._layout.ready.get()
+        return self._layout
 
     # ------------------------------------------------------------------ search
     def _check_query(self, x, k):
@@ -278,6 +274,7 @@ class IVFPQIndex(IdContainer):
                    _lib.current_stream(dev)))
         return out
 
+    @on_index_device
     def search(self, x, k=1, return_address=False, return_keys=False):
         """IVFPQIndex.search (IVFPQIndex.py:469-524): x [d_vector, n_query] fp32 on the index device
         -> (topk_values [n_query, k] fp32 descending, topk_ids [n_query, k] int64[, topk_address])."""
@@ -288,6 +285,7 @@ class IVFPQIndex(IdContainer):
                                                                                   temperature, *out),
                             return_address=return_address, return_keys=return_keys)
 
+    @on_index_device
     def range_search(self, x, threshold, return_address=False, max_results=1 << 26):
         """Every item that search would score for a query with a score above `threshold`: x [d_vector, n_query] fp32 on
         the index device, threshold a float or a 0-d tensor (rounded once to fp32; NaN raises ValueError)
@@ -318,6 +316,7 @@ class IVFPQIndex(IdContainer):
                                              _lib.current_stream(dev)))
         return _range.collect(run, nq, max_results, self._address2id, return_address, dev)
 
+    @on_index_device
     def search_cells(self, x, cells, base_sims=None, n_probe_list=None, k=1, return_address=False, return_keys=False):
         """IVFPQIndex.search_cells, non-residual branch (IVFPQIndex.py:407-467)."""
         x = self._check_query(x, k)
@@ -355,6 +354,7 @@ class IVFPQIndex(IdContainer):
             peer_ptrs, n_peers, my_slot, *ws), outputs=False)
 
     # ------------------------------------------------------------------ build side (see build.py)
+    @on_index_device
     def train(self, x, force_retrain=False, seed=0):
         if self.vq_codec.is_trained and self.pq_codec.is_trained and not force_retrain:
             self.print_message("index is already trained", 1)                 # IVFPQIndex.py:235-238
@@ -362,10 +362,12 @@ class IVFPQIndex(IdContainer):
         from . import build
         build.train(self, x, seed=seed)
 
+    @on_index_device
     def add(self, x, ids=None, return_address=False):
         from . import build
         return build.add(self, x, ids, return_address)
 
+    @on_index_device
     def remove(self, ids=None, address=None):
         """CellContainer.remove (CellContainer.py:369-393) as it is documented to behave (README.md:60-66: "virtually
         remove vectors ... ignores ids that don't exist").  The shipped reference returns early whenever fewer items
@@ -377,6 +379,7 @@ class IVFPQIndex(IdContainer):
         from . import build
         build.container_remove(self, ids, address)
 
+    @on_index_device
     def encode(self, x):
         """IVFPQIndex.encode (IVFPQIndex.py:262-287): x [d_vector, n] -> PQ codes [n_subvectors, n] uint8
         (residual index: (pq_code of x - vq centroid, vq_code), IVFPQIndex.py:281-284)."""
@@ -390,6 +393,7 @@ class IVFPQIndex(IdContainer):
         sub = x.reshape(self.n_subvectors, self.d_subvector, x.shape[1])
         return build._assign(sub, self.pq_codec.codebook).to(torch.uint8)
 
+    @on_index_device
     def decode(self, code):
         """IVFPQIndex.decode (IVFPQIndex.py:289-314) -> PQCodec.decode (PQCodec.py:113-130): [M, n] u8 -> [d, n] f32
         (residual index: x = (pq_code, vq_code) -> vq centroid + decoded residual)."""

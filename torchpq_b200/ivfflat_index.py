@@ -18,7 +18,7 @@ import torch
 
 from . import _lib, _range
 from ._lib import lib, check, ptr
-from .modules import Codec, IdContainer, _fingerprint
+from .modules import Codec, IdContainer, StreamCache, _fingerprint, on_index_device
 
 
 class IVFFlatIndex(IdContainer):
@@ -81,6 +81,7 @@ class IVFFlatIndex(IdContainer):
         self._refresh_max_id()
 
     # ------------------------------------------------------------------ build side (build.py, shared with IVFPQIndex)
+    @on_index_device
     def train(self, x, force_retrain=False, seed=0):
         """The coarse half of IVFPQIndex.train (build.train_coarse): k-means on x (normalised for cosine)."""
         if self.vq_codec.is_trained and not force_retrain:
@@ -91,6 +92,7 @@ class IVFFlatIndex(IdContainer):
         self.vq_codec.set_codebook(vq)
         self._state_changed()
 
+    @on_index_device
     def add(self, x, ids=None, return_address=False, chunk: int = 1 << 20):
         """x [d, n] fp32: cell = exact assignment of x (normalised for cosine, as IVFPQIndex.add); the stored vector is
         x itself.  Placement, holes and expansion are IVFPQIndex's (build.container_add)."""
@@ -109,6 +111,7 @@ class IVFFlatIndex(IdContainer):
         codes = x.view(torch.uint8).view(self.d_vector, x.shape[1], 4).permute(0, 2, 1).reshape(self.code_size, x.shape[1])
         return build.container_add(self, codes.contiguous(), cells, ids, return_address)   # calls _state_changed
 
+    @on_index_device
     def remove(self, ids=None, address=None):
         """As IVFPQIndex.remove: removed slots become holes that search skips and the next add fills first;
         ``_cell_size`` is not decremented."""
@@ -132,8 +135,8 @@ class IVFFlatIndex(IdContainer):
             table = torch.empty(max(1, cap), dtype=torch.float32, device=dev)
             check(lib.tpq_flat_norms(ptr(self._storage), cap, self.d_vector, cap, _lib.METRIC[self.distance], ptr(table),
                                      _lib.current_stream(dev)))
-            self._norms = (key, table)
-        return self._norms[1]
+            self._norms = (key, StreamCache(table, dev))
+        return self._norms[1].get()
 
     def _check_query(self, x, k):
         assert x.dim() == 2 and x.shape[0] == self.d_vector
@@ -165,12 +168,14 @@ class IVFFlatIndex(IdContainer):
                     _lib.current_stream(dev)))
         return out
 
+    @on_index_device
     def search(self, x, k=1, return_address=False):
         """x [d_vector, n_query] fp32 on the index device -> (values [n_query, k] fp32 descending, ids [n_query, k]
         int64[, address]).  Probes as IVFPQIndex.search (n_probe, use_smart_probing, smart_probing_temperature)."""
         x = self._check_query(x, k)
         return self._search(x, k, int(self.n_probe), None, None, return_address)
 
+    @on_index_device
     def range_search(self, x, threshold, return_address=False, max_results=1 << 26):
         """Every item that search would score for a query with a score above `threshold`: x [d_vector, n_query] fp32 on
         the index device, threshold a float or a 0-d tensor (rounded once to fp32; NaN raises ValueError)
@@ -203,6 +208,7 @@ class IVFFlatIndex(IdContainer):
                         ws_bytes, _lib.current_stream(dev)))
         return _range.collect(run, nq, max_results, self._address2id, return_address, dev)
 
+    @on_index_device
     def search_cells(self, x, cells, n_probe_list=None, k=1, return_address=False):
         """As IVFPQIndex.search_cells: cells [n_query, n_probe] int64 probe lists, n_probe_list [n_query] int64
         (default n_probe)."""

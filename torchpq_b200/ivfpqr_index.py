@@ -28,7 +28,7 @@ import torch
 from . import _lib
 from ._lib import lib, check, ptr
 from .index import IVFPQIndex
-from .modules import Codec
+from .modules import Codec, on_index_device
 
 
 class IVFPQRIndex(IVFPQIndex):
@@ -74,6 +74,7 @@ class IVFPQRIndex(IVFPQIndex):
         y2 = self._pq_encode(x, self.pq_rerank_codec.codebook, self.n_subvectors_rerank)
         return torch.cat([y1, y2], dim=0)
 
+    @on_index_device
     def encode(self, x):
         """IVFPQRIndex.encode (IVFPQRIndex.py:128-154): x [d_vector, n] -> [M + Mr, n] u8, the PQ code and the re-rank
         code (of the PQ code's residual with use_residual)."""
@@ -84,6 +85,7 @@ class IVFPQRIndex(IVFPQIndex):
             x = fn.normalize(x)
         return self._encode(x)
 
+    @on_index_device
     def decode(self, code):
         """IVFPQRIndex.decode (IVFPQRIndex.py:156-175): [M + Mr, n] u8 -> [d, n] f32, the re-rank decode plus, with
         use_residual, the PQ decode."""
@@ -95,6 +97,7 @@ class IVFPQRIndex(IVFPQIndex):
         return y
 
     # ------------------------------------------------------------------ build side
+    @on_index_device
     def train(self, x, force_retrain=False, seed=0):
         """IVFPQRIndex.train (IVFPQRIndex.py:108-126) as meant: VQ and PQ on x (cosine: on the normalised x), then the
         re-rank codec on x - decode_pq(encode_pq(x)) with use_residual, else on x.  Each k-means runs build.fit with its
@@ -125,6 +128,7 @@ class IVFPQRIndex(IVFPQIndex):
         self.pq_rerank_codec.set_codebook(pqr)
         self._state_changed()
 
+    @on_index_device
     def add(self, x, ids=None, return_address=False, chunk: int = 1 << 20):
         """IVFPQRIndex.add (IVFPQRIndex.py:177-222): VQ cells and the [M + Mr] code of each column, stored by the
         container add of IVFPQIndex."""
@@ -141,6 +145,7 @@ class IVFPQRIndex(IVFPQIndex):
         return build.container_add(self, torch.cat(codes_l, 1), torch.cat(cells_l, 0), ids, return_address)
 
     # ------------------------------------------------------------------ search
+    @on_index_device
     def search(self, x, k=1, return_address=False):
         """x [d_vector, n_query] fp32 -> (values [n_query, k] fp32 descending, ids [n_query, k] i64[, address]).
         First pass: the IVFPQ scan's k1 = min(1024, max(k, ceil(k_factor * k))) best addresses.  Second pass
@@ -152,6 +157,7 @@ class IVFPQRIndex(IVFPQIndex):
         _, _, cand = IVFPQIndex.search(self, x, k1, return_address=True)
         return self.rerank(x, cand, k, return_address)
 
+    @on_index_device
     def rerank(self, x, candidates, k, return_address=False):
         """The second pass alone (tpq_rerank): x [d_vector, n_query] fp32, candidates [n_query, k1] i64 addresses
         (-1 = none), k <= k1 <= 1024 -> (values, ids[, address]) [n_query, k]."""

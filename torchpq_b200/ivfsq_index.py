@@ -20,7 +20,7 @@ from . import _lib
 from ._lib import lib, check, ptr
 from .codec import SQCodec
 from .ivfflat_index import IVFFlatIndex
-from .modules import _fingerprint
+from .modules import StreamCache, _fingerprint, on_index_device
 
 _NORM_CHUNK = 1 << 16            # slots decoded at a time by the norm table's build
 
@@ -44,6 +44,7 @@ class IVFSQIndex(IVFFlatIndex):
         return torch.zeros(self.d_vector * self.bits // 32, cap, 4, dtype=torch.uint8, device=dev)
 
     # ------------------------------------------------------------------ build side
+    @on_index_device
     def train(self, x, force_retrain=False, seed=0):
         """IVFFlatIndex.train (build.train_coarse), then sq_codec.train on the same x (normalised for cosine)."""
         if self.vq_codec.is_trained and not force_retrain:
@@ -63,6 +64,7 @@ class IVFSQIndex(IVFFlatIndex):
         """sq_codec.decode: [d, n] codes -> [d, n] fp32."""
         return self.sq_codec.decode(code)
 
+    @on_index_device
     def add(self, x, ids=None, return_address=False, chunk: int = 1 << 20):
         """x [d, n] fp32: cell = exact assignment of x (normalised for cosine), code = sq_codec.encode of that same x.
         Placement, holes and expansion are IVFPQIndex's (build.container_add)."""
@@ -122,8 +124,8 @@ class IVFSQIndex(IVFFlatIndex):
                 n = min(_NORM_CHUNK, cap - s)
                 x = self.decode(self._codes_at(slice(s, s + n)).contiguous())
                 check(lib.tpq_flat_norms(ptr(x), n, d, n, _lib.METRIC[self.distance], ptr(table[s:]), st))
-            self._norms = (key, table)
-        return self._norms[1]
+            self._norms = (key, StreamCache(table, dev))
+        return self._norms[1].get()
 
     def _store_args(self):
         lo, rg = self.sq_codec._bounds(self._storage.device)               # None for 16 bits

@@ -8,6 +8,8 @@ the same buffer names, so a ``state_dict`` saved by ``torchpq.index.IVFPQIndex``
 """
 from __future__ import annotations
 
+import functools
+
 import torch
 import torch.nn as nn
 
@@ -35,8 +37,54 @@ class StateModule(nn.Module):
         pass
 
 
+def on_device(device_of):
+    """Decorator: run the function with the CUDA device of its data made current, ``device_of(*args, **kwargs)``.
+    The library launches every kernel on the current device, into the stream it is given, and reads the current
+    device's SM count; a stream of another device makes the launch fail.  So an index on cuda:1 works while cuda:0
+    is current.  Data already on the current device, or not on a CUDA device at all (the function's own checks reject
+    it), runs as is."""
+    def wrap(fn):
+        @functools.wraps(fn)
+        def run(*args, **kwargs):
+            dev = device_of(*args, **kwargs)
+            if dev.type != "cuda" or dev.index is None or dev.index == torch.cuda.current_device():
+                return fn(*args, **kwargs)
+            with torch.cuda.device(dev):
+                return fn(*args, **kwargs)
+        return run
+    return wrap
+
+
+on_index_device = on_device(lambda self, *a, **k: self._address2id.device)   # a method of an index
+on_data_device = on_device(lambda x, *a, **k: x.device)                      # a function of a tensor
+
+
 def _fingerprint(*tensors):
     return tuple((t.data_ptr(), t._version, tuple(t.shape)) if t is not None else None for t in tensors)
+
+
+class StreamCache:
+    """A device-side cache (a norm table, a scan layout) filled by kernels on the stream current at construction, and
+    read from any stream.  Construct it after the cache's last kernel: it records an event there, and ``get`` makes a
+    reader on another stream wait on that event, so a search never reads a half-built cache.  The wait is skipped while
+    the reader's stream is capturing a CUDA graph: ``torch.cuda.graph`` synchronises the device before it captures, so
+    the cache is complete by then, and a capture may not wait on an event recorded outside it."""
+
+    def __init__(self, value, device):
+        # built inside a capture, the cache would live in the graph's pool and be filled only on replay, and eager
+        # searches would then read it unfilled
+        assert not torch.cuda.is_current_stream_capturing(), \
+            "a cache was built inside a CUDA graph capture: run the call once eagerly before capturing it"
+        self.value = value
+        self._stream = torch.cuda.current_stream(device)
+        self._ready = torch.cuda.Event()
+        self._ready.record(self._stream)
+
+    def get(self):
+        cur = torch.cuda.current_stream(self._stream.device)
+        if cur.cuda_stream != self._stream.cuda_stream and not torch.cuda.is_current_stream_capturing():
+            cur.wait_event(self._ready)
+        return self.value
 
 
 class IdContainer(StateModule):
