@@ -299,6 +299,23 @@ int tpq_rerank(const float* x_dn, int d, int nq, const int64_t* candidates, int 
                int k, const int64_t* address2id, float* values, int64_t* ids, int64_t* address,
                void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ exact refine (RefineFlatIndex.search, second pass)
+ * candidates [nq, k1] i64: addresses into vectors (-1 = none; any address outside [0, n) is dropped too), k <= k1 <=
+ * 1024; a candidate listed twice is scored twice.  vectors [n, d] f32 row-major, n < 2^32.  Per candidate y, exactly in
+ * fp32:
+ *   EUCLIDEAN acc = fmaf(-dif, dif, acc), dif = x_e - y_e, e ascending from +0, exactly d terms (tpq_max_sim's arithmetic);
+ *   COSINE    acc = fmaf(x_e, y_e, acc) on x / (||x|| + 1e-9) (as tpq_normalize_columns), y as stored (the caller
+ *             stores normalised vectors);
+ * i.e. the value equals tpq_max_sim(x_q, y), the arithmetic of tpq_rerank.  -> values [nq, k] f32 descending (-inf
+ * padded), ids [nq, k] i64 (address2id[address], -1 padded), address [nq, k] i64 (nullable, -1 padded); order score
+ * descending, then address ascending.  Arguments are checked before any launch (k and k1, metric, sizes, workspace,
+ * pointers; vectors may be NULL when n == 0); nq == 0 returns at once.  ws: at least
+ * tpq_refine_flat_workspace_bytes(d, nq, k) bytes. */
+size_t tpq_refine_flat_workspace_bytes(int d, int nq, int k);
+int tpq_refine_flat(const float* x_dn, int d, int nq, const int64_t* candidates, int k1,
+                    const float* vectors, int64_t n, int metric, int k, const int64_t* address2id,
+                    float* values, int64_t* ids, int64_t* address, void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------ k-means / codec neighbours of the path
  * tpq_max_sim: MultiKMeans assignment, MaxSimCuda(dim=2, mode "tn") (kernels/MaxSimCuda.py:184-238,
  *   kernels/cuda/max_sim.cu:182-309; caller clustering/MultiKMeans.py:314-333):

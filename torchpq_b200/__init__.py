@@ -1,6 +1,7 @@
 """torchpq_b200 -- H100-native (sm_90a) IVFPQ search path behind torchpq.index.IVFPQIndex.search(), IVFPQ search
 re-ranked on a second PQ code (IVFPQRIndex), exact flat search (FlatIndex), inverted-file search with exact distances
-(IVFFlatIndex), inverted-file search over scalar-quantized vectors (IVFSQIndex, codec.SQCodec), row-wise top-k (topk = fn.Topk()), and k-means
+(IVFFlatIndex), inverted-file search over scalar-quantized vectors (IVFSQIndex, codec.SQCodec), exact fp32 re-ranking of any
+of these indexes' candidates (RefineFlatIndex), row-wise top-k (topk = fn.Topk()), and k-means
 (clustering.KMeans / MultiKMeans).
 
 Importing this package loads ``libtpq_b200.so``; there is no CPU / PyTorch fallback.
@@ -11,6 +12,7 @@ from .flat_index import FlatIndex
 from .ivfpqr_index import IVFPQRIndex
 from .ivfflat_index import IVFFlatIndex
 from .ivfsq_index import IVFSQIndex
+from .refine_index import RefineFlatIndex
 from . import codec
 from . import fn
 from . import clustering
@@ -19,4 +21,4 @@ from .patch import patch, unpatch
 
 topk = fn.Topk()                     # torchpq.topk (torchpq/__init__.py:22)
 
-__all__ = ["IVFPQIndex", "IVFPQRIndex", "IVFFlatIndex", "IVFSQIndex", "FlatIndex", "codec", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "topk", "patch", "unpatch"]
+__all__ = ["IVFPQIndex", "IVFPQRIndex", "IVFFlatIndex", "IVFSQIndex", "FlatIndex", "RefineFlatIndex", "codec", "ScanLayout", "KMeans", "MultiKMeans", "clustering", "fn", "topk", "patch", "unpatch"]

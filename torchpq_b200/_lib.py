@@ -83,6 +83,8 @@ SIGNATURES = {
     "tpq_flat_search": (_I, [_P, _I, _I, _P, _I64, _I64, _P, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
     "tpq_rerank_workspace_bytes": (_SZ, [_I, _I, _I]),
     "tpq_rerank": (_I, [_P, _I, _I, _P, _I, _P, _I64, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
+    "tpq_refine_flat_workspace_bytes": (_SZ, [_I, _I, _I]),
+    "tpq_refine_flat": (_I, [_P, _I, _I, _P, _I, _P, _I64, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
     "tpq_topk_workspace_bytes": (_SZ, [_I64, _I64, _I, _I]),
     "tpq_topk": (_I, [_P, _I64, _I64, _I, _I, _P, _P, _P, _SZ, _P]),
     "tpq_ivfflat_workspace_bytes": (_SZ, [_I, _I, _I, _I, _I]),

@@ -18,11 +18,13 @@
 //      the thread runs the d-long fmaf chain, its codebook lookups `cb[e * 256 + code]` gathered from shared memory;
 //   3. warp w sorts query w's k1 keys, 64 at a time, into a kp-slot list (merge_staged + warp_merge_run) and writes its
 //      first k keys; tpq_merge_topk with one part decodes them into values, addresses and ids.
+// Steps 1 and 3 are query_tile.cuh's, shared with refine.cu.
 // Codebooks: each is d * 1 KB (128 KB at d = 128), so at d = 128 only one fits in shared memory beside the tile.  The
 // re-rank codebook is staged first because every score reads it; the first-level one only with use_residual.  A
 // codebook that does not fit is read through the read-only cache.  CTAs persist across tiles so that the staging is paid
 // once per CTA, not once per tile.
 #include "gemm_tile.cuh"
+#include "query_tile.cuh"
 
 extern "C" int tpq_merge_topk(const uint64_t* keys_in, int nq, int n_parts, int k, const int64_t* address2id,
                               int64_t capacity, float* values, int64_t* ids, int64_t* address, void* stream);
@@ -108,10 +110,7 @@ rerank_kernel(const RerankArgs A) {
   for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
     const int q0 = t * A.qt, nqt = min(A.qt, A.nq - q0);
     __syncthreads();                                                         // the previous tile's x and lists are read
-    for (int i = tid; i < nqt * d; i += kRrThreads) {
-      const int q = i / d, e = i - q * d;
-      xs[i] = A.x[(size_t)e * A.nq + q0 + q];
-    }
+    load_query_tile<kRrThreads>(A, xs, d, q0, nqt, tid);
     __syncthreads();
     for (int p = tid; p < nqt * k1; p += kRrThreads) {
       const int q = p / k1;
@@ -137,16 +136,7 @@ rerank_kernel(const RerankArgs A) {
       keys[p] = key;
     }
     __syncthreads();
-    if (warp < nqt) {
-      uint64_t* list = lists + (size_t)warp * A.kp;
-      for (int i = lane; i < A.kp; i += 32) list[i] = 0ull;
-      __syncwarp();
-      const uint64_t* kq = keys + (size_t)warp * k1;
-      for (int c0 = 0; c0 < k1; c0 += 64)
-        merge_staged<2>(kq + c0, min(k1 - c0, 64), A.kp, lane, [&](const auto& x) { warp_merge_run(list, A.kp, x, lane); });
-      uint64_t* dst = A.keys_out + (size_t)(q0 + warp) * A.k;
-      for (int i = lane; i < A.k; i += 32) dst[i] = list[i];
-    }
+    select_query_tile(A, keys, lists, k1, nqt, q0, warp, lane);
   }
 }
 

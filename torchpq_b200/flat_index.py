@@ -19,7 +19,7 @@ import torch
 
 from . import _lib, _range
 from ._lib import lib, check, ptr
-from .modules import IdContainer, StreamCache, _fingerprint, on_index_device
+from .modules import IdContainer, StreamCache, _fingerprint, live_prefix, on_index_device, prefix_remove
 
 _DISTANCE = {"euclidean": "euclidean", "l2": "euclidean", "cosine": "cosine", "angular": "cosine",
              "inner": "inner", "dot": "inner"}                     # FlatIndex.py:31-40
@@ -60,9 +60,7 @@ class FlatIndex(IdContainer):
         """Reference semantics (CustomModule.py:14-23), then the state the reference keeps outside its buffers:
         ``n_items`` = the live slots (address2id >= 0), which must be a prefix of the store, and ``max_id``."""
         super().load_state_dict(state_dict, strict)
-        live = self._address2id >= 0
-        n = int(live.sum().item())
-        assert bool(live[:n].all().item()), "the live slots of a flat index must be the prefix [0, n_items)"
+        n = live_prefix(self._address2id)
         assert self._storage.shape == (self.d_vector, self.capacity, 1)
         self._n_items = n
         self._refresh_max_id()
@@ -140,21 +138,12 @@ class FlatIndex(IdContainer):
             address = address.to(self._address2id.device)
         else:
             raise RuntimeError("Need either ids or address")
-        n_items = self._n_items
-        address = address[(0 <= address) & (address < n_items)].unique(sorted=True)
-        n_removed = address.shape[0]
+        n_removed, dst, src, tail = prefix_remove(self._address2id, address, self._n_items)
         if n_removed == 0:
             return 0
-        tail = slice(n_items - n_removed, n_items)
-        self._address2id[address] = -1
-        keep = self._address2id[tail] != -1                              # surviving items of the tail, ascending
-        n_move = int(keep.sum().item())
-        dst = address[:n_move]                                           # the removed slots below the tail
-        self._storage[:, dst] = self._storage[:, tail][:, keep].clone()
-        self._address2id[dst] = self._address2id[tail][keep].clone()
+        self._storage[:, dst] = self._storage[:, src].clone()
         self._storage[:, tail] = 0
-        self._address2id[tail] = -1
-        self._n_items = n_items - n_removed
+        self._n_items -= n_removed
         self._state_changed()
         return n_removed
 

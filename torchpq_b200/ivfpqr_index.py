@@ -21,14 +21,12 @@ Not covered, each with an error: ``drop_reference_layout`` / ``dist.distribute``
 """
 from __future__ import annotations
 
-import math
-
 import torch
 
 from . import _lib
 from ._lib import lib, check, ptr
 from .index import IVFPQIndex
-from .modules import Codec, on_index_device
+from .modules import Codec, k1_of, on_index_device
 
 
 class IVFPQRIndex(IVFPQIndex):
@@ -153,7 +151,7 @@ class IVFPQRIndex(IVFPQIndex):
         -- the k best kept; a value equals fn.max_sim(x_q, decode(codes)) bit for bit."""
         x = self._check_query(x, k)
         assert self.pq_rerank_codec.is_trained, "codec is not trained"
-        k1 = min(1024, max(k, math.ceil(self.k_factor * k)))
+        k1 = k1_of(k, self.k_factor)
         _, _, cand = IVFPQIndex.search(self, x, k1, return_address=True)
         return self.rerank(x, cand, k, return_address)
 

@@ -9,6 +9,7 @@ the same buffer names, so a ``state_dict`` saved by ``torchpq.index.IVFPQIndex``
 from __future__ import annotations
 
 import functools
+import math
 
 import torch
 import torch.nn as nn
@@ -141,6 +142,41 @@ class IdContainer(StateModule):
         address = torch.ones_like(ids) * -1
         address[mask] = self._id2address[ids[mask]]
         return address
+
+
+def live_prefix(address2id):
+    """The number of live slots (address2id >= 0) of a store whose live slots must be the prefix [0, n_items), as
+    FlatIndex and RefineFlatIndex keep it; a checkpoint whose live slots are not a prefix is refused."""
+    live = address2id >= 0
+    n = int(live.sum().item())
+    assert bool(live[:n].all().item()), "the live slots of a flat index must be the prefix [0, n_items)"
+    return n
+
+
+def prefix_remove(address2id, address, n_items):
+    """FlatContainer.remove's rule (FlatContainer.py:160-190) for a store whose live slots are the prefix [0, n_items):
+    the surviving items of the last n_removed slots move, in ascending order, into the removed slots below them.
+    Addresses outside the live prefix are ignored.  Updates address2id in place and returns (n_removed, dst, src, tail):
+    the caller moves its rows src -> dst and clears the slots of `tail` (a slice)."""
+    address = address[(0 <= address) & (address < n_items)].unique(sorted=True)
+    n_removed = address.shape[0]
+    if n_removed == 0:
+        return 0, None, None, None
+    tail = slice(n_items - n_removed, n_items)
+    address2id[address] = -1
+    keep = address2id[tail] != -1                                    # surviving items of the tail, ascending
+    n_move = int(keep.sum().item())
+    dst = address[:n_move]                                           # the removed slots below the tail
+    src = torch.arange(n_items - n_removed, n_items, dtype=torch.long, device=address2id.device)[keep]
+    address2id[dst] = address2id[src].clone()
+    address2id[tail] = -1
+    return n_removed, dst, src, tail
+
+
+def k1_of(k, k_factor):
+    """The first pass's depth of a re-ranked search (IVFPQRIndex, RefineFlatIndex): k1 = min(1024, max(k,
+    ceil(k_factor * k))) candidates, re-scored exactly and cut to k."""
+    return min(1024, max(k, math.ceil(k_factor * k)))
 
 
 class _Centroids(StateModule):
