@@ -191,6 +191,36 @@ int tpq_ivfflat_search(const float* x_dn, int d, int nq, const float* vq_codeboo
                        int k, const int64_t* address2id, float* values, int64_t* ids, int64_t* address,
                        void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------ IVF search over 4-bit PQ codes (IVFPQ4Index)
+ * The store is the IVFPQ cell container read in place (no scan layout): storage [M/8, capacity, 4] u8, 4-byte aligned,
+ * code m of a slot in nibble m & 1 (low first) of byte m >> 1, so word g holds sub-quantizers 8g .. 8g+7; is_empty
+ * [capacity], cell_start / cell_size [n_cells], address2id [capacity]; capacity < 2^32.  vq_codebook [d, n_cells],
+ * pq_codebook [M, d/M, 16]; M a multiple of 8, at most 256 (TPQ_ERR_UNSUPPORTED beyond).
+ * part2 (nullable; EUCLIDEAN only): residual IVFPQ, [n_cells, M, 16] f32, the cell half of each cell's LUT,
+ *   (c_m . p * -2) - nrm * nrm (lut.cuh's part 2 entry).
+ * cells == NULL: the coarse probe of tpq_ivfpq_search runs inside (x normalised by tpq_normalize_columns for COSINE;
+ *   n_probe <= n_cells, n_probe > 1024 TPQ_ERR_UNSUPPORTED; residual base = the probe similarities); else cells
+ *   [nq, n_probe] i64, n_probe_list [nq] i64 and, residual, base_sims [nq, n_probe] f32 as for tpq_ivfpq_search_cells
+ *   (x used as given; smart and temperature unused).
+ * Visited: tpq_ivfpq_search's rule, the first max(1, min((int)n_probe_list[q], n_probe)) entries (residual: max(0, ...)),
+ *   skipping cells outside [0, n_cells) and an entry whose cell_start equals the previous entry's; a visited cell's live
+ *   slots of [cell_start, cell_start + cell_size) are scored.  LUT [M][16] per query (lut.cuh's entries, from +0 fmaf
+ *   chains over the d/M dimensions):  EUCLIDEAN ((2 dot) - |x_m|^2) - |p|^2   COSINE dot   residual: (2 dot) + part2[cell]
+ *   (one fp32 add per entry).  Score = base + acc, acc = LUT[m][code_m] summed over m ascending from +0 in fp32, base =
+ *   the cell's coarse similarity (residual) or +0.
+ * -> values [nq, k] f32 descending (-inf padded), ids [nq, k] i64 (address2id[address], -1 padded), address [nq, k] i64
+ *   (nullable, -1 padded).  Order: score descending, then address ascending; independent of the batch and its slicing.
+ *   Arguments are checked before any launch; nq == 0 returns at once.  ws: at least
+ *   tpq_ivfpq4_workspace_bytes(d, nq, n_cells, n_probe, k) bytes. */
+size_t tpq_ivfpq4_workspace_bytes(int d, int nq, int n_cells, int n_probe, int k);
+int tpq_ivfpq4_search(const float* x_dn, int d, int M, int nq, int metric, const uint8_t* storage,
+                      const uint8_t* is_empty, const int64_t* cell_start, const int64_t* cell_size,
+                      const int64_t* address2id, int64_t capacity, int n_cells, const float* vq_codebook,
+                      const float* pq_codebook, const float* part2, const int64_t* cells,
+                      const int64_t* n_probe_list, const float* base_sims, int n_probe, int smart,
+                      float temperature, int k, float* values, int64_t* ids, int64_t* address, void* ws,
+                      size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------ scalar quantization (SQCodec, IVFSQIndex)
  * tpq_sq_encode: x_dn [d, n] f32 -> out [d, n]: u8 for bits 8, fp16 for bits 16, f32 (a copy) for bits 32.
  * tpq_sq_decode: codes [d, n] in the same types -> out_dn [d, n] f32.  lower / range [d] f32 (bits 8 only, NULL

@@ -101,6 +101,9 @@ SIGNATURES = {
                                       _P, _I64, _P, _P, _SZ, _P]),
     "tpq_ivfsq_range_search": (_I, [_P, _I, _I, _P, _I, _P, _I, _P, _P, _I64, _P, _P, _P, _P, _I, _P, _P, _I, _I, _F,
                                     _F, _P, _P, _I64, _P, _P, _SZ, _P]),
+    "tpq_ivfpq4_workspace_bytes": (_SZ, [_I, _I, _I, _I, _I]),
+    "tpq_ivfpq4_search": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I64, _I, _P, _P, _P, _P, _P, _P, _I, _I, _F,
+                               _I, _P, _P, _P, _P, _SZ, _P]),
     "tpq_ivfpq_range_workspace_bytes": (_SZ, [_IX, _I, _I]),
     "tpq_ivfpq_range_search": (_I, [_IX, _P, _P, _P, _P, _I, _I, _I, _F, _F, _P, _P, _I64, _P, _P, _SZ, _P]),
 }

@@ -211,8 +211,9 @@ def container_add(index, codes: torch.Tensor, cells: torch.Tensor, ids=None, ret
     write = fn.get_write_address(cells, ioa, index._cell_start, index._cell_size, index._cell_capacity, prefix)
     ix = lay.cindex if in_sync else _lib.TpqIndex()
     if not in_sync:
-        # no scanned code without a scan layout: 4, the smallest n_subvectors tpq_store_codes takes, for a flat store
-        ix.n_subvectors, ix.n_cells, ix.capacity = getattr(index, "n_subvectors", 4), index.n_cells, index.capacity
+        # no scanned code without a scan layout: 4, the smallest n_subvectors tpq_store_codes takes (it then reads only
+        # code_size), for any store, IVFPQ4Index's too, whose code_size is n_subvectors / 2
+        ix.n_subvectors, ix.n_cells, ix.capacity = 4, index.n_cells, index.capacity
         ix.code_size = index.code_size
         ix.shard_world = 1
     ix.cell_start = index._cell_start.data_ptr()

@@ -1,5 +1,5 @@
 """RefineFlatIndex: any index of this package, its candidates re-ranked exactly on stored fp32 vectors (Faiss:
-``IndexRefineFlat``).
+``IndexRefineFlat``): FlatIndex, IVFPQIndex, IVFPQRIndex, IVFFlatIndex, IVFSQIndex or IVFPQ4Index.
 
 ``search(x, k)`` asks the base index for k1 = min(1024, max(k, ceil(k_factor * k))) candidate ids per query, maps each
 to its row of a row-major fp32 store through the id map, scores it exactly (``tpq_refine_flat``, csrc/refine.cu) and
